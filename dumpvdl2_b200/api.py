@@ -35,6 +35,10 @@ class _Config(C.Structure):
                 ("flags", C.c_uint32), ("n_inflight", C.c_uint32), ("n_streams", C.c_uint32), ("reserved", C.c_uint32 * 4)]
 
 
+class _Receiver(C.Structure):
+    _fields_ = [("centerfreq", C.c_uint32), ("n_channels", C.c_uint32)]
+
+
 class _Frame(C.Structure):
     _fields_ = [("channel", C.c_uint32), ("freq", C.c_uint32), ("burst_seq", C.c_uint32), ("idx", C.c_int32),
                 ("data", C.POINTER(C.c_uint8)), ("len", C.c_uint32), ("synd_weight", C.c_uint32),
@@ -70,6 +74,7 @@ def load_library():
                            "(nvcc, sm_90a). There is no CPU fallback for the demodulator path.")
     L = C.CDLL(LIB_PATH)
     L.vdl2gpu_create.argtypes = [C.POINTER(_Config), C.POINTER(C.c_void_p)]
+    L.vdl2gpu_create_receivers.argtypes = [C.POINTER(_Config), C.POINTER(_Receiver), C.c_uint32, C.POINTER(C.c_void_p)]
     L.vdl2gpu_destroy.argtypes = [C.c_void_p]
     L.vdl2gpu_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
@@ -330,3 +335,57 @@ class Vdl2Channels:
         n = (C.c_uint64 * 5)()
         _check(self.L, self.L.vdl2gpu_get_kernel_ms(self.h, ms, n), "vdl2gpu_get_kernel_ms")
         return dict(K0=(ms[0], n[0]), K1=(ms[1], n[1]), K2a=(ms[2], n[2]), K2=(ms[3], n[3]), K3=(ms[4], n[4]))
+
+
+class Vdl2Receivers(Vdl2Channels):
+    """R receivers on one H100, each with its own centre frequency and its own channels; every receiver decodes exactly
+    as one reference process tuned to its centre would.  Channel numbers are global: receiver r owns channels
+    channels_of(r).  The receivers advance in lock step: submit() takes one equal-length buffer per receiver."""
+
+    def __init__(self, sample_rate, oversample, sample_fmt, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1,
+                 flags=0, n_inflight=4):
+        """receivers: list of (centerfreq, [channel freqs...])"""
+        self.L = load_library()
+        self.receivers = [(int(cf), [int(f) for f in fr]) for cf, fr in receivers]
+        self.n_receivers = self.n_streams = len(self.receivers)
+        self.freqs = np.ascontiguousarray([f for _, fr in self.receivers for f in fr], dtype=np.uint32)
+        self.n_channels = int(self.freqs.size)
+        self._first = np.concatenate([[0], np.cumsum([len(fr) for _, fr in self.receivers], dtype=np.int64)]).astype(np.int64)
+        self.sample_fmt = sample_fmt
+        rx = (_Receiver * max(self.n_receivers, 1))()
+        for r, (cf, fr) in enumerate(self.receivers):
+            rx[r].centerfreq, rx[r].n_channels = cf, len(fr)
+        cfg = _Config()
+        cfg.sample_rate, cfg.oversample, cfg.sample_fmt = sample_rate, oversample, sample_fmt
+        cfg.n_channels = self.n_channels
+        cfg.freqs = self.freqs.ctypes.data_as(C.POINTER(C.c_uint32))
+        cfg.max_ppm, cfg.max_chunk_bytes, cfg.device, cfg.flags, cfg.n_inflight = max_ppm, max_chunk_bytes, device, flags, n_inflight
+        cfg.n_streams = self.n_receivers
+        self.h = C.c_void_p()
+        _check(self.L, self.L.vdl2gpu_create_receivers(C.byref(cfg), rx, self.n_receivers, C.byref(self.h)), "vdl2gpu_create_receivers")
+        self._frames = []
+        self._cb = _FRAME_CB(self._on_frame)
+
+    def channels_of(self, r):
+        """global channel numbers of receiver r"""
+        return range(int(self._first[r]), int(self._first[r + 1]))
+
+    def receiver_of(self, channel):
+        if not 0 <= channel < self.n_channels:
+            raise IndexError(f"channel {channel} out of range")
+        return int(np.searchsorted(self._first, channel, side="right")) - 1
+
+    def submit(self, bufs):
+        """one buffer per receiver, all of the same length in bytes"""
+        if len(bufs) != self.n_receivers:
+            raise Vdl2GpuError(f"{len(bufs)} buffers for {self.n_receivers} receivers")
+        parts = [np.ascontiguousarray(b).view(np.uint8).reshape(-1) for b in bufs]
+        if any(p.size != parts[0].size for p in parts):
+            raise Vdl2GpuError("the receivers' buffers differ in length")
+        return self._submit(np.concatenate(parts), self.sample_fmt)
+
+    def process_chunked(self, bufs, chunk_bytes):
+        """each receiver's whole stream (equal lengths), submitted chunk_bytes per receiver at a time"""
+        parts = [np.ascontiguousarray(b).view(np.uint8).reshape(-1) for b in bufs]
+        for off in range(0, parts[0].size, chunk_bytes):
+            self.submit([p[off:off + chunk_bytes] for p in parts])

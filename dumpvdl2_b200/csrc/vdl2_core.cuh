@@ -1112,4 +1112,83 @@ VDL2_HD uint16_t vdl2_crc16(const uint8_t *p, uint32_t len) {
 	return (uint16_t)crc;
 }
 
+/* ------------------------------------------------------------------------------------------------
+ * Channel layout: slot -> channel -> receiver, and the tile geometry of the receiver-group K1
+ * ---------------------------------------------------------------------------------------------- */
+/* slot (index into every per-channel array) -> public channel number and activity: a warp holds `lanes` channels in its
+ * first `lanes` lanes (the first full_warps warps) or lanes - 1 (the others); see the slot mapping in vdl2_host.cu */
+VDL2_HD bool vdl2_slot_channel(uint32_t slot, uint32_t lanes, uint32_t full_warps, uint32_t n_ch, uint32_t &chan) {
+	const uint32_t lane = slot & 31u, w = slot >> 5;
+	const uint32_t mine = w < full_warps ? lanes : lanes - 1u;                 /* channels of this warp */
+	chan = (w < full_warps ? w * lanes : full_warps * lanes + (w - full_warps) * (lanes - 1u)) + lane;
+	return lane < mine && chan < n_ch;
+}
+
+/* Multi-receiver context (vdl2gpu_create_receivers): receiver r owns channels [rx_first[r], rx_first[r + 1]), every
+ * receiver at least one.  Returns the receiver of a channel (binary search over the n_rx + 1 boundaries). */
+VDL2_HD uint32_t vdl2_rx_of_channel(uint32_t chan, const uint32_t *rx_first, uint32_t n_rx) {
+	uint32_t lo = 0, hi = n_rx;                   /* rx_first[lo] <= chan < rx_first[hi] */
+	while(hi - lo > 1u) {
+		const uint32_t mid = (lo + hi) >> 1;
+		if(rx_first[mid] <= chan) lo = mid; else hi = mid;
+	}
+	return lo;
+}
+
+#define VDL2_RX_K1_BLOCK 128u                         /* slots per block of the receiver-group K1 */
+/* Shared memory of one receiver-group K1 block: with one K2 block (~116 KB) it must fit the 228 KB of an SM, or the
+ * K2(c) || K1(c+1) schedule of the pipeline (one block of each per SM) breaks */
+#define VDL2_RX_K1_SMEM_BUDGET (110u * 1024u)
+#define VDL2_RX_K1_LUT_BYTES (257u * 8u * 16u)         /* the eight NCO table copies */
+
+/* Every 128-slot block covers a contiguous channel range, hence a contiguous receiver range.  Fills slot_rx[n_blocks * 128]
+ * (receiver of the slot's channel; an inactive slot gets its block's first receiver) and block_rx[n_blocks][2] = {first
+ * receiver, number of receivers G} (G = 0 for a block without channels); returns the largest G. */
+VDL2_HD uint32_t vdl2_rx_layout(uint32_t n_blocks, uint32_t lanes, uint32_t full_warps, uint32_t n_ch, const uint32_t *rx_first,
+		uint32_t n_rx, uint32_t *slot_rx, uint32_t *block_rx) {
+	uint32_t g_max = 0;
+	for(uint32_t b = 0; b < n_blocks; b++) {
+		uint32_t first = 0xFFFFFFFFu, last = 0;
+		for(uint32_t t = 0; t < VDL2_RX_K1_BLOCK; t++) {
+			uint32_t chan;
+			if(!vdl2_slot_channel(b * VDL2_RX_K1_BLOCK + t, lanes, full_warps, n_ch, chan)) continue;
+			const uint32_t r = vdl2_rx_of_channel(chan, rx_first, n_rx);
+			slot_rx[b * VDL2_RX_K1_BLOCK + t] = r;
+			if(first == 0xFFFFFFFFu) first = r;
+			last = r;
+		}
+		const uint32_t g = first == 0xFFFFFFFFu ? 0u : last - first + 1u;
+		if(first == 0xFFFFFFFFu) first = 0;
+		for(uint32_t t = 0; t < VDL2_RX_K1_BLOCK; t++) {
+			uint32_t chan;
+			if(!vdl2_slot_channel(b * VDL2_RX_K1_BLOCK + t, lanes, full_warps, n_ch, chan)) slot_rx[b * VDL2_RX_K1_BLOCK + t] = first;
+		}
+		block_rx[2 * b] = first;
+		block_rx[2 * b + 1] = g;
+		if(g > g_max) g_max = g;
+	}
+	return g_max;
+}
+
+/* float2 elements per staged receiver row for a tile of T samples: room for T + 2 (the odd-phase shift and the odd
+ * trailing sample), rounded up to 2 mod 16.  Even keeps every row 16-byte aligned for the bulk copy; 2 mod 16 starts row
+ * r 4 r banks further on, so up to eight receivers of one warp read different banks. */
+VDL2_HD uint32_t vdl2_rx_tile_stride(uint32_t T) { return T + 2u + (16u - T % 16u) % 16u; }
+
+VDL2_HD uint32_t vdl2_rx_k1_smem_bytes(uint32_t G, uint32_t T) {
+	return 2u * G * vdl2_rx_tile_stride(T) * 8u + VDL2_RX_K1_LUT_BYTES + 16u;     /* two tile buffers, table, two mbarriers */
+}
+
+/* T for blocks of up to G receivers: the most whole decimation groups, an even number of samples (16-byte bulk copies),
+ * that keep vdl2_rx_k1_smem_bytes(G, T) within VDL2_RX_K1_SMEM_BUDGET; 0 if not even one fits */
+VDL2_HD uint32_t vdl2_rx_tile_samples(uint32_t G, uint32_t oversample) {
+	if(G == 0) G = 1;
+	const uint32_t avail = VDL2_RX_K1_SMEM_BUDGET - VDL2_RX_K1_LUT_BYTES - 16u;
+	const uint32_t r_max = avail / (16u * G);
+	if(r_max < 2u + 2u) return 0;
+	const uint32_t r = r_max - (r_max - 2u) % 16u;                  /* largest row stride <= r_max that is 2 mod 16 */
+	const uint32_t step = (oversample & 1u) ? 2u * oversample : oversample;
+	return (r - 2u) / step * step;
+}
+
 #endif

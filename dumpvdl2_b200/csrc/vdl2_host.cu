@@ -20,6 +20,7 @@
 #include <string>
 #include <vector>
 #include "../../include/vdl2gpu.h"
+#include "vdl2_core.cuh"
 #include "vdl2_kernels.h"
 #include "vdl2_types.h"
 #include "vdl2_tables_host.h"
@@ -85,6 +86,9 @@ struct vdl2gpu_ctx {
 	int n_sms = 0;                                      /* read from the device at create */
 	uint32_t n_streams = 1, ch_per_stream = 0;          /* independent-streams mode: n_streams > 1, channels [s*C, (s+1)*C) on stream s */
 	bool lane_streams = false;                          /* C == 1: samples kept time-major across streams, one lane per stream in K1 */
+	bool receivers = false;                             /* vdl2gpu_create_receivers: n_streams receivers, each with its own centre and channels */
+	uint32_t *d_slot_rx = nullptr, *d_block_rx = nullptr;   /* receivers: vdl2_rx_layout tables (fixed at create) */
+	uint32_t rx_tile = 0, rx_max = 0;                   /* receivers: samples per staged tile, most receivers of one K1 block */
 	uint32_t raw_bytes = 0;                             /* size of each slot's raw staging buffers (allocated on the first host submit) */
 	int k1_variant = 2, k2_variant = 5, k2a_mode = 1;   /* A/B knobs (VDL2GPU_K1_VARIANT, VDL2GPU_K2_VARIANT, VDL2GPU_K2A), read at create */
 	bool use_graphs = true;
@@ -129,8 +133,8 @@ static uint32_t dphi_for(uint32_t centerfreq, uint32_t freq, uint32_t rate) {   
 	return (uint32_t)(int)(((float)centerfreq - (float)freq) / (float)rate * 256.0f * 65536.0f);
 }
 
-static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, uint32_t n_ch, uint32_t n_chp, uint32_t lanes, uint32_t full_warps,
-		std::vector<uint32_t> &k1, std::vector<uint32_t> &k2);
+static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, uint32_t n_ch, uint32_t n_chp,
+		uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2);
 /* channel -> slot: the first full_warps warps hold `lanes` channels each, the others lanes - 1 */
 static inline uint32_t slot_of(uint32_t ch, uint32_t lanes, uint32_t full_warps) {
 	const uint32_t head = full_warps * lanes;
@@ -188,6 +192,7 @@ static int free_ctx(vdl2gpu_ctx *c) {
 	cudaFree(c->d_k1); cudaFree(c->d_k2);
 	cudaFree(c->d_counters); cudaFree(c->d_ready); cudaFree(c->d_ring); cudaFree(c->d_pool); cudaFree(c->d_free);
 	cudaFree(c->d_ctl); cudaFree(c->d_events); cudaFree(c->d_block_trace);
+	cudaFree(c->d_slot_rx); cudaFree(c->d_block_rx);
 	if(c->ev_input_ready) cudaEventDestroy(c->ev_input_ready);
 	if(c->ev_input_consumed) cudaEventDestroy(c->ev_input_consumed);
 	if(c->ev_drain) cudaEventDestroy(c->ev_drain);
@@ -201,7 +206,8 @@ static int free_ctx(vdl2gpu_ctx *c) {
 	return VDL2GPU_OK;
 }
 
-static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c) {
+/* rx / n_rx: the receivers of a multi-receiver context (vdl2gpu_create_receivers, validated there), NULL / 0 otherwise */
+static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_receiver *rx = nullptr, uint32_t n_rx = 0) {
 	int ndev = 0;
 	cudaError_t e = cudaGetDeviceCount(&ndev);
 	if(e != cudaSuccess || ndev == 0) {
@@ -220,12 +226,13 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c) {
 	}
 	KL(vdl2_kernels_init_device(c->device));             /* per device: function attributes do not carry over */
 	c->cfg = *cfg;
-	c->n_streams = cfg->n_streams ? cfg->n_streams : 1u;
+	c->receivers = rx != nullptr;
+	c->n_streams = c->receivers ? n_rx : cfg->n_streams ? cfg->n_streams : 1u;
 	c->cfg.n_streams = c->n_streams;
-	c->lane_streams = c->n_streams > 1 && c->n_streams == cfg->n_channels;     /* one stream per channel */
+	c->lane_streams = !c->receivers && c->n_streams > 1 && c->n_streams == cfg->n_channels;     /* one stream per channel */
 	if(c->lane_streams) {
 		c->ch_per_stream = 1;
-	} else if(c->n_streams > 1) {
+	} else if(c->n_streams > 1 && !c->receivers) {      /* (receivers: any channel count each, see the receiver tables below) */
 		if(cfg->n_channels % c->n_streams != 0 || (cfg->n_channels / c->n_streams) % 32u != 0) {
 			snprintf(g_last_error, sizeof(g_last_error), "independent-streams mode needs n_channels = n_streams x C with C = 1 or a multiple of 32 (got %u channels, %u streams)",
 					cfg->n_channels, c->n_streams);
@@ -250,7 +257,7 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c) {
 		const char *e = getenv("VDL2GPU_FUSE_PHASE");
 		const int k2v = c->k2_variant & 0xFF;
 		c->fuse_phase = (e && atoi(e) != 0) && c->k2a_mode == 1 && !(k2v >= 0 && k2v <= 4) && c->stages == 2
-			&& vdl2_k1_fuses_phase(cfg->oversample, c->ch_per_stream, (cfg->flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant);
+			&& vdl2_k1_fuses_phase(cfg->oversample, c->ch_per_stream, (cfg->flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->receivers ? 1 : 0);
 	}
 	if(cfg->flags & (VDL2GPU_FLAG_NO_GRAPH | VDL2GPU_FLAG_TRACE)) c->use_graphs = false;
 	c->freqs.assign(cfg->freqs, cfg->freqs + cfg->n_channels);
@@ -267,7 +274,7 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c) {
 	 * sub-partitions, they are dealt out evenly over ALL of them: every warp holds floor or ceil of n_ch / (4 x SMs)
 	 * channels instead of 32 (31 or 32 at 16384 channels on 132 SMs), each of the two kernels launches exactly one block
 	 * per SM, every block lives for the whole kernel, and every SM looks the same to the scheduler. */
-	if(cfg->n_streams <= 1 || cfg->n_streams == cfg->n_channels) {
+	if(c->receivers || cfg->n_streams <= 1 || cfg->n_streams == cfg->n_channels) {
 		const uint32_t warps_all = 4u * (uint32_t)c->n_sms;
 		if(c->n_ch > 16u * warps_all && c->n_ch <= 32u * warps_all) {
 			const char *e = getenv("VDL2GPU_BALANCE");
@@ -281,6 +288,7 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c) {
 	const uint32_t max_bytes = cfg->max_chunk_bytes ? cfg->max_chunk_bytes : (1u << 20);
 	c->cfg.max_chunk_bytes = max_bytes;
 	c->max_pairs = max_bytes / (cfg->sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
+	if(c->receivers) c->max_pairs = (c->max_pairs + 1u) & ~1u;     /* even row stride: every receiver row of the plane starts 16-byte aligned */
 	c->max_dec = c->max_pairs / cfg->oversample + 2;
 	if((uint64_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp >= (1ull << 32)) {
 		snprintf(g_last_error, sizeof(g_last_error), "%u channels x %u decimated samples per chunk exceed the 32-bit element index of the kernels; "
@@ -343,8 +351,24 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c) {
 	CU(cudaMemset(c->d_ring, 0, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
 	CU(cudaMemset(c->d_pool, 0, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
 
-	std::vector<uint32_t> k1, k2;
-	initial_state(c->cfg, c->freqs.data(), c->n_ch, c->n_chp, c->lanes, c->full_warps, k1, k2);
+	std::vector<uint32_t> k1, k2, centres;
+	if(c->receivers) {
+		/* every channel mixes against its own receiver's centre (src/demod.c:385); the slot -> receiver tables K1 stages by */
+		std::vector<uint32_t> rx_first(n_rx + 1, 0);
+		for(uint32_t r = 0; r < n_rx; r++) {
+			rx_first[r + 1] = rx_first[r] + rx[r].n_channels;
+			centres.insert(centres.end(), rx[r].n_channels, rx[r].centerfreq);
+		}
+		const uint32_t n_blocks = (c->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
+		std::vector<uint32_t> slot_rx((size_t)n_blocks * VDL2_RX_K1_BLOCK), block_rx(2 * (size_t)n_blocks);
+		c->rx_max = vdl2_rx_layout(n_blocks, c->lanes, c->full_warps, c->n_ch, rx_first.data(), n_rx, slot_rx.data(), block_rx.data());
+		c->rx_tile = vdl2_rx_tile_samples(c->rx_max, cfg->oversample);
+		CU(cudaMalloc(&c->d_slot_rx, slot_rx.size() * 4));
+		CU(cudaMalloc(&c->d_block_rx, block_rx.size() * 4));
+		CU(cudaMemcpy(c->d_slot_rx, slot_rx.data(), slot_rx.size() * 4, cudaMemcpyHostToDevice));
+		CU(cudaMemcpy(c->d_block_rx, block_rx.data(), block_rx.size() * 4, cudaMemcpyHostToDevice));
+	}
+	initial_state(c->cfg, c->freqs.data(), c->receivers ? centres.data() : nullptr, c->n_ch, c->n_chp, c->lanes, c->full_warps, k1, k2);
 	CU(cudaMemcpy(c->d_k1, k1.data(), k1.size() * 4, cudaMemcpyHostToDevice));
 	CU(cudaMemcpy(c->d_k2, k2.data(), k2.size() * 4, cudaMemcpyHostToDevice));
 	std::vector<int32_t> fl(c->n_slots);
@@ -378,6 +402,35 @@ extern "C" int vdl2gpu_create(const vdl2gpu_config *cfg, vdl2gpu_ctx **out) {
 	}
 	vdl2gpu_ctx *c = new vdl2gpu_ctx();
 	int rc = create_impl(cfg, c);
+	if(rc != VDL2GPU_OK) { free_ctx(c); *out = nullptr; return rc; }
+	*out = c;
+	return VDL2GPU_OK;
+}
+
+extern "C" int vdl2gpu_create_receivers(const vdl2gpu_config *cfg, const vdl2gpu_receiver *rx, uint32_t n_rx, vdl2gpu_ctx **out) {
+	const char *why = nullptr;
+	uint64_t sum = 0;
+	if(!cfg || !out || !cfg->freqs || cfg->n_channels == 0 || cfg->oversample == 0 || cfg->sample_fmt > 1
+			|| cfg->sample_rate != (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * cfg->oversample) why = "bad vdl2gpu_config (sample_rate must be 105000*oversample)";
+	else if(!rx || n_rx == 0) why = "no receivers";
+	else if(n_rx > 65535u) why = "more than 65535 receivers (one K0 grid row each)";
+	else if(cfg->n_streams != 0 && cfg->n_streams != n_rx) why = "n_streams must be 0 or the number of receivers";
+	else if(cfg->oversample != 20 && cfg->oversample != 10 && cfg->oversample != 13) why = "receivers need oversample 20, 10 or 13 (the rates the receiver-group K1 is built for)";
+	else if(cfg->flags & VDL2GPU_FLAG_K1_SCALAR) why = "VDL2GPU_FLAG_K1_SCALAR is not available with receivers";
+	else {
+		for(uint32_t r = 0; r < n_rx && !why; r++) {
+			if(rx[r].n_channels == 0) why = "a receiver has no channels";
+			sum += rx[r].n_channels;
+		}
+		if(!why && sum != cfg->n_channels) why = "the receivers' channel counts do not add up to n_channels";
+	}
+	if(why) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_create_receivers: %s", why);
+		if(out) *out = nullptr;
+		return VDL2GPU_EINVAL;
+	}
+	vdl2gpu_ctx *c = new vdl2gpu_ctx();
+	int rc = create_impl(cfg, c, rx, n_rx);
 	if(rc != VDL2GPU_OK) { free_ctx(c); *out = nullptr; return rc; }
 	*out = c;
 	return VDL2GPU_OK;
@@ -549,6 +602,7 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	p1.one = 1.0f; p1.neg_one = -1.0f; p1.two = 2.0f;
 	p1.trace_blocks = c->d_block_trace; p2.trace_blocks = c->d_block_trace;
 	p1.ch_per_stream = c->ch_per_stream; p1.stream_stride = c->lane_streams ? c->n_chp : c->max_pairs; p1.ca = ca;
+	p1.slot_rx = c->d_slot_rx; p1.block_rx = c->d_block_rx; p1.rx_tile = c->rx_tile; p1.rx_max = c->rx_max;
 	p1.phase = c->fuse_phase ? c->d_phase2[pb] : nullptr; p1.phase_prev = c->d_phase2[pb ^ 1]; p1.prev_n_dec = prev_n_dec;
 	/* the default walk (variant 5) computes the four magnitudes a block needs from the staged samples: no magnitude plane */
 	const bool need_mag = (c->k2_variant & 0xFF) >= 0 && (c->k2_variant & 0xFF) <= 4;
@@ -748,7 +802,7 @@ extern "C" int vdl2gpu_submit(vdl2gpu_ctx *c, const void *iq, uint32_t len) {
 
 extern "C" int vdl2gpu_submit_planar_s16(vdl2gpu_ctx *c, const int16_t *xi, const int16_t *xq, uint32_t n_pairs) {
 	if(!c || ((!xi || !xq) && n_pairs)) return VDL2GPU_EINVAL;
-	if(c->cfg.sample_fmt != VDL2GPU_FMT_S16_LE || c->n_streams != 1) return VDL2GPU_EINVAL;
+	if(c->cfg.sample_fmt != VDL2GPU_FMT_S16_LE || c->n_streams != 1 || c->receivers) return VDL2GPU_EINVAL;
 	if(n_pairs == 0) return VDL2GPU_OK;
 	if((uint64_t)n_pairs * 4u > c->cfg.max_chunk_bytes) return VDL2GPU_ETOOBIG;
 	CU(cudaSetDevice(c->device));
@@ -1146,15 +1200,16 @@ extern "C" uint32_t vdl2gpu_stage_row_stride(uint32_t n_channels) { return (n_ch
 
 /* initial per-channel state: vdl2_channel_init + demod_reset (src/demod.c:205-220,379-392), process_samples locals
  * (src/demod.c:289-298); shared by the batch context and the stage stubs */
-static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, uint32_t n_ch, uint32_t n_chp, uint32_t lanes, uint32_t full_warps,
-		std::vector<uint32_t> &k1, std::vector<uint32_t> &k2) {
+static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, uint32_t n_ch, uint32_t n_chp,
+		uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2) {
 	k1.assign((size_t)K1_NFIELDS * n_chp, 0u); k2.assign((size_t)K2_NFIELDS * n_chp, 0u);
 	auto fbits = [](float f) { uint32_t u; memcpy(&u, &f, 4); return u; };
 	for(uint32_t chan = 0; chan < n_ch; chan++) {
 		const uint32_t ch = slot_of(chan, lanes, full_warps);          /* index into the per-channel planes */
 		/* a channel on the centre frequency skips the mixer in the reference (src/demod.c:312); with a zero
 		 * phase step the table gives cos = 1, sin = 0 and the products are exact, so no branch is needed */
-		k1[(size_t)K1_DPHI * n_chp + ch] = (cfg.centerfreq != freqs[chan]) ? dphi_for(cfg.centerfreq, freqs[chan], cfg.sample_rate) : 0u;
+		const uint32_t centre = centres ? centres[chan] : cfg.centerfreq;     /* centres: per channel, multi-receiver context */
+		k1[(size_t)K1_DPHI * n_chp + ch] = (centre != freqs[chan]) ? dphi_for(centre, freqs[chan], cfg.sample_rate) : 0u;
 		k2[(size_t)K2_MAG_NF * n_chp + ch] = fbits(2.0f);
 		k2[(size_t)K2_PHERR1 * n_chp + ch] = fbits(1000.f);
 		k2[(size_t)K2_PHERR2 * n_chp + ch] = fbits(1000.f);
@@ -1195,7 +1250,7 @@ extern "C" int vdl2gpu_stage_create(const vdl2gpu_config *cfg, uint32_t max_dec,
 	st->d_ready = reinterpret_cast<uint32_t *>(b + L.ready); st->d_ctl = reinterpret_cast<vdl2_queue_ctl *>(b + L.ctl);
 	st->d_events = b + L.events;
 	std::vector<uint32_t> k1, k2;
-	initial_state(st->cfg, st->freqs.data(), st->n_ch, st->n_chp, 32u, 0xFFFFFFFFu, k1, k2);
+	initial_state(st->cfg, st->freqs.data(), nullptr, st->n_ch, st->n_chp, 32u, 0xFFFFFFFFu, k1, k2);
 	std::vector<int32_t> fl(st->n_slots);
 	for(uint32_t i = 0; i < st->n_slots; i++) fl[i] = (int32_t)i;
 	vdl2_queue_ctl ctl;

@@ -34,15 +34,6 @@ __device__ __forceinline__ int vdl2_trace_begin(vdl2_block_trace *t, uint32_t ke
 }
 __device__ __forceinline__ void vdl2_trace_end(vdl2_block_trace *t, int k) { if(k >= 0) t->rec[k].t_end = vdl2_globaltimer(); }
 
-/* slot (index into every per-channel array) -> public channel number and activity: a warp holds `lanes` channels in its
- * first `lanes` lanes */
-__device__ __forceinline__ bool vdl2_slot_channel(uint32_t slot, uint32_t lanes, uint32_t full_warps, uint32_t n_ch, uint32_t &chan) {
-	const uint32_t lane = slot & 31u, w = slot >> 5;
-	const uint32_t mine = w < full_warps ? lanes : lanes - 1u;                 /* channels of this warp */
-	chan = (w < full_warps ? w * lanes : full_warps * lanes + (w - full_warps) * (lanes - 1u)) + lane;
-	return lane < mine && chan < n_ch;
-}
-
 /* ------------------------------------------------------------------------------------------------
  * K0: sample conversion.  Output: float2 {re, im} per complex sample (src/demod.c:339-365).
  * ---------------------------------------------------------------------------------------------- */
@@ -608,6 +599,154 @@ __global__ void __launch_bounds__(K1L_BLOCK) k1_mix_iir_decimate_lanes(vdl2_k1_p
 		}
 		k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
 	}
+}
+
+/* ------------------------------------------------------------------------------------------------
+ * K1, many receivers in one context (vdl2gpu_create_receivers): R receivers, each with its own centre frequency and any
+ * number of channels.  K0 writes the sample plane float2[n_rx][stream_stride] (one row per receiver, 8 B per
+ * receiver-sample); a 128-slot block covers a contiguous channel range, i.e. the G receivers block_rx[b] = {first, G}.
+ * Every tile stages the same window of T = rx_tile samples of each of them into s_tiles[2][G][vdl2_rx_tile_stride(T)]:
+ * one cp.async.bulk per receiver row, issued by the lanes of warp 0, all completing on the tile's mbarrier.  Each lane
+ * reads its receiver's row (the lanes of one receiver broadcast).  The row stride is even, so every row of the plane has
+ * the same 16-byte phase and one `mis` serves all of them.  Block shape, NCO table copies and per-lane arithmetic
+ * (k1_packed_step, the software-pipelined group body, the symmetric-tap form) are those of the packed kernel, so every
+ * decimated sample is the reference's bit for bit.
+ * ---------------------------------------------------------------------------------------------- */
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
+	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tma_copy(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+			:: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+
+template<int OS, bool SYM>
+__global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_groups(vdl2_k1_params p) {
+	constexpr int NLUT = 8, LA = 10, MA = 5;
+	extern __shared__ __align__(128) unsigned char k1g_smem[];
+	const uint32_t T = p.rx_tile, R = vdl2_rx_tile_stride(T), TG = T / OS;
+	const uint32_t rx0 = p.block_rx[2 * blockIdx.x], G = p.block_rx[2 * blockIdx.x + 1];
+	float2 *s_tiles = reinterpret_cast<float2 *>(k1g_smem);                                         /* [2][G][R] */
+	float4 *s_lut = reinterpret_cast<float4 *>(k1g_smem + (size_t)2 * G * R * 8);                   /* [257][8] */
+	uint64_t *s_bar = reinterpret_cast<uint64_t *>(k1g_smem + (size_t)2 * G * R * 8 + 257 * NLUT * 16);
+	const uint32_t tid = threadIdx.x, lane = tid & 31u;
+	const int trace_k = tid == 0 ? vdl2_trace_begin(p.trace_blocks, 1) : -1;
+	const uint32_t ch = blockIdx.x * VDL2_RX_K1_BLOCK + tid;
+	uint32_t chan;
+	const bool active = vdl2_slot_channel(ch, p.lanes, p.full_warps, p.n_ch, chan);
+	const uint32_t row = p.slot_rx[ch] - rx0;                                /* this lane's receiver within the block */
+	const uint32_t n_pairs = p.ca ? p.ca->n_pairs : p.n_pairs, cnt0 = p.ca ? p.ca->cnt0 : p.cnt0;
+	const size_t stride = p.stream_stride;
+	const float2 *plane = p.samples + (size_t)rx0 * stride;                  /* the block's first receiver */
+	const float2 *samples = plane + (size_t)row * stride;
+	for(uint32_t i = tid; i < 257 * NLUT; i += VDL2_RX_K1_BLOCK) s_lut[i] = p.lut[i / NLUT];
+	const float4 *lut = s_lut + (tid & (NLUT - 1));
+	const uint32_t lane_bytes = (tid & (NLUT - 1)) * 16u;
+	if(tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
+	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
+	uint32_t phi = 0, dphi = 0;
+	if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
+	u64 x1 = f2_pack(xr1, xi1), x2 = f2_pack(xr2, xi2), y1 = f2_pack(yr1, yi1), y2 = f2_pack(yr2, yi2);
+	k1_packed_consts c;
+	c.ONE = f2_pack(p.one, p.one); c.SGN = f2_pack(p.neg_one, p.one);
+	c.A0 = f2_pack(p.a0, p.a0); c.A1 = f2_pack(p.a1, p.a1); c.A2 = f2_pack(p.a2, p.a2);
+	c.B1 = f2_pack(p.b1, p.b1); c.B2 = f2_pack(p.b2, p.b2); c.TWO = f2_pack(p.two, p.two);
+	c.one = p.one; c.neg_one = p.neg_one;
+	__syncthreads();
+
+	uint32_t cnt = cnt0, m = 0, pos = 0;
+	const uint32_t head = min(n_pairs, (OS - cnt0 % OS) % OS);
+	if(active) {
+		for(; pos < head; pos++) {
+			u64 y0 = k1_packed_step(samples[pos], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
+			if(++cnt == OS) { cnt = 0; p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0)); m++; }
+		}
+	}
+	pos = head;
+	m = (cnt0 + head) / OS;
+	cnt = (cnt0 + head) % OS;
+	u64 P1 = f2_mul(c.A0, x1), P2 = f2_mul(c.A0, x2);
+	const uint32_t n_groups = (n_pairs - pos) / OS;
+	const uint32_t n_tiles = (n_groups + TG - 1) / TG;
+	/* odd first body sample: every row is fetched from one sample earlier and read from element 1 on, as in the packed kernel */
+	const uint32_t mis = (uint32_t)((reinterpret_cast<uintptr_t>(plane + pos) >> 3) & 1u);
+	auto request_tile = [&](uint32_t t, uint32_t buf) {              /* warp 0 */
+		const uint32_t n = min(TG, n_groups - t * TG) * OS + mis;
+		const uint32_t bytes = (n & ~1u) * (uint32_t)sizeof(float2);
+		if(lane == 0) mbar_expect_tx(&s_bar[buf], G * bytes);
+		__syncwarp();
+		const size_t off = head + (size_t)t * T - mis;
+		for(uint32_t r = lane; r < G; r += 32) {
+			const float2 *src = plane + (size_t)r * stride + off;
+			float2 *dst = s_tiles + ((size_t)buf * G + r) * R;
+			tma_copy(dst, src, bytes, &s_bar[buf]);
+			if(n & 1u) dst[n - 1] = src[n - 1];
+		}
+	};
+	if(tid < 32)
+		for(uint32_t t = 0; t < 2 && t < n_tiles; t++) request_tile(t, t);
+	__syncthreads();
+	auto tile_loop = [&](auto MIS) {
+	for(uint32_t g0 = 0, tile = 0; g0 < n_groups; g0 += TG, tile++) {
+		const uint32_t ng = min(TG, n_groups - g0);
+		const float2 *s_tile = s_tiles + ((size_t)(tile & 1u) * G + row) * R + decltype(MIS)::value;
+		mbar_wait(&s_bar[tile & 1u], (tile >> 1) & 1u);
+		if(active) {
+			for(uint32_t g = 0; g < ng; g++) {
+				const float2 *sp = &s_tile[g * OS];
+				u64 y0 = 0;
+				float2 S[OS];
+				float4 E[OS];
+				float FR[OS];
+				u64 X0[OS];
+#pragma unroll
+				for(int k = -LA; k < OS; k++) {
+					const int kl = k + LA, km = k + MA;
+					if(kl < OS) {
+						const uint32_t ph = phi + (uint32_t)kl * dphi;
+						E[kl] = k1_lut_entry<NLUT>(s_lut, ph, lane_bytes);
+						FR[kl] = (float)(ph & 0xFFFFu);
+						S[kl] = sp[kl];
+					}
+					if(km >= 0 && km < OS) {
+						const u64 CS = f2_fma(f2_mul(f2_pack(E[km].z, E[km].w), f2_pack(FR[km], FR[km])), c.ONE, f2_pack(E[km].x, E[km].y));
+						X0[km] = k1_mix(S[km], CS, c);
+					}
+					if(k >= 0) {
+						const u64 x0 = X0[k];
+						u64 r;
+						if(SYM) {
+							const u64 P0 = f2_mul(c.A0, x0);
+							r = f2_fma(P0, c.ONE, f2_fma(P1, c.TWO, P2));
+							P2 = P1; P1 = P0;
+						} else {
+							const u64 t = f2_fma(f2_mul(c.A1, x1), c.ONE, f2_mul(c.A2, x2));
+							r = f2_fma(f2_mul(c.A0, x0), c.ONE, t);
+						}
+						const u64 u = f2_fma(f2_mul(c.B1, y1), c.ONE, f2_mul(c.B2, y2));
+						y0 = f2_fma(r, c.ONE, u);
+						x2 = x1; x1 = x0; y2 = y1; y1 = y0;
+					}
+				}
+				phi += (uint32_t)OS * dphi;
+				p.dec[(size_t)(m + g) * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0));
+			}
+		}
+		m += ng;
+		pos += ng * OS;
+		__syncthreads();                                           /* every warp is done with this buffer */
+		if(tid < 32 && tile + 2 < n_tiles) request_tile(tile + 2, tile & 1u);
+	}
+	};
+	if(mis) tile_loop(std::integral_constant<int, 1>{}); else tile_loop(std::integral_constant<int, 0>{});
+	if(active) {
+		for(; pos < n_pairs; pos++) {
+			u64 y0 = k1_packed_step(samples[pos], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
+			if(++cnt == OS) { cnt = 0; p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0)); m++; }
+		}
+		k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+	}
+	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);
 }
 
 /* ------------------------------------------------------------------------------------------------
@@ -1185,6 +1324,10 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		cudaFuncSetAttribute(k1_mix_iir_decimate_lanes<20, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, K1L_SMEM_BYTES);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_lanes<10, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, K1L_SMEM_BYTES);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_lanes<10, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, K1L_SMEM_BYTES);
+#define K1G_SETUP(OS, SYM) do { vdl2_set_carveout(k1_mix_iir_decimate_groups<OS, SYM>, pct); \
+		cudaFuncSetAttribute(k1_mix_iir_decimate_groups<OS, SYM>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_K1_SMEM_BUDGET); } while(0)
+		K1G_SETUP(20, true); K1G_SETUP(20, false); K1G_SETUP(10, true); K1G_SETUP(10, false); K1G_SETUP(13, true); K1G_SETUP(13, false);
+#undef K1G_SETUP
 		vdl2_set_carveout(k2a_phase_mag<true>, pct);
 		vdl2_set_carveout(k2a_phase_mag_warps<true>, pct);
 		vdl2_set_carveout(k2a_phase_mag_warps<false>, pct);
@@ -1232,8 +1375,8 @@ static void k1_launch_packed(const vdl2_k1_params *p, int variant, bool sym, cud
 	else k1_mix_iir_decimate_packed<OS, BLOCK, 10, false><<<blocks, BLOCK, 0, st>>>(*p);
 }
 
-extern "C" int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, int force_scalar, int variant) {
-	if(force_scalar || variant == 0 || variant == 8 || ch_per_stream == 1) return 0;
+extern "C" int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, int force_scalar, int variant, int receivers) {
+	if(receivers || force_scalar || variant == 0 || variant == 8 || ch_per_stream == 1) return 0;
 	if(ch_per_stream != 0 && ch_per_stream % K1_BLOCK != 0) return 0;
 	return oversample == 20 || oversample == 10 || oversample == 13;
 }
@@ -1243,6 +1386,19 @@ extern "C" int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, 
 extern "C" int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st) {
 	if(p->n_pairs == 0 || p->n_ch == 0) return 0;
 	const bool sym = (p->a1 == 2.0f * p->a0) && (p->a2 == p->a0) && variant != 4;
+	if(p->slot_rx) {                                  /* multi-receiver context: samples are float2[n_rx][stream_stride] */
+		const uint32_t blocks = (p->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
+		const uint32_t smem = vdl2_rx_k1_smem_bytes(p->rx_max, p->rx_tile);
+		if(p->rx_tile == 0 || p->rx_tile % p->oversample != 0 || smem > VDL2_RX_K1_SMEM_BUDGET) return (int)cudaErrorInvalidValue;
+#define K1G_GO(OS) do { if(sym) k1_mix_iir_decimate_groups<OS, true><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p); \
+		else k1_mix_iir_decimate_groups<OS, false><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p); } while(0)
+		if(p->oversample == 20) K1G_GO(20);
+		else if(p->oversample == 10) K1G_GO(10);
+		else if(p->oversample == 13) K1G_GO(13);
+		else return (int)cudaErrorInvalidValue;
+#undef K1G_GO
+		return (int)cudaGetLastError();
+	}
 	if(p->ch_per_stream == 1) {                       /* one stream per channel: samples are float2[n_pairs][stream_stride] */
 		const uint32_t blocks = (p->n_chp + K1L_BLOCK - 1) / K1L_BLOCK;
 		if(p->oversample == 20) {

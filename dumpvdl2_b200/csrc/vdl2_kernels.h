@@ -56,6 +56,12 @@ typedef struct {
 	float *phase;
 	const float *phase_prev;
 	uint32_t prev_n_dec;         /* overridden by ca->prev_n_dec */
+	/* multi-receiver context (vdl2gpu_create_receivers; NULL otherwise): `samples` is float2[n_rx][stream_stride], receiver-major;
+	 * slot_rx[slot] = receiver of the slot's channel, block_rx[2 b] / [2 b + 1] = first receiver / number of receivers of
+	 * 128-slot block b (vdl2_rx_layout); every tile stages rx_tile samples of each of them, at most rx_max per block */
+	const uint32_t *slot_rx;
+	const uint32_t *block_rx;
+	uint32_t rx_tile, rx_max;
 } vdl2_k1_params;
 
 typedef struct {
@@ -124,8 +130,8 @@ int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t fmt, const 
 		uint32_t raw_stride, uint32_t out_stride, uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *ca, cudaStream_t st);
 int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st);
 /* whether vdl2_launch_k1 with these arguments runs a kernel that honours p->phase (the pipelined packed kernel with
- * 128-channel blocks); everything else leaves the phase plane to K2a */
-int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, int force_scalar, int variant);
+ * 128-channel blocks); everything else, the receiver-group kernel included, leaves the phase plane to K2a */
+int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, int force_scalar, int variant, int receivers);
 int vdl2_launch_copy_hist(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k2a(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k2a_warps(const vdl2_k2a_params *p, cudaStream_t st);

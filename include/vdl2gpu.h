@@ -129,6 +129,18 @@ typedef struct vdl2gpu_ctx vdl2gpu_ctx;
 int vdl2gpu_abi_version(void);
 int vdl2gpu_device_count(void);
 int vdl2gpu_create(const vdl2gpu_config *cfg, vdl2gpu_ctx **out);
+/* Many receivers in one context: receiver r has its own tuning and its own channels, exactly as if it were one reference
+ * process (vdl2_channel_init(rx[r].centerfreq, freq, ...) per channel, src/demod.c:379-392).  cfg->freqs lists the
+ * channels receiver by receiver (receiver r owns the next rx[r].n_channels entries), cfg->n_channels is their sum,
+ * cfg->n_streams is 0 or n_rx and cfg->centerfreq is ignored.  Channel numbers (frames, counters, read_dec, events) index
+ * cfg->freqs.  All receivers share sample rate and format and advance in lock step: vdl2gpu_submit / vdl2gpu_submit_device
+ * take the n_rx buffers of `len` bytes back to back (receiver 0 first); vdl2gpu_submit_planar_s16 is not available.
+ * n_rx <= 65535; oversample 20, 10 or 13; VDL2GPU_FLAG_K1_SCALAR is refused. */
+typedef struct {
+	uint32_t centerfreq;         /* Hz: this receiver's tuning (src/demod.c:385 uses it for every channel of the receiver) */
+	uint32_t n_channels;         /* >= 1; this receiver's channels are the next n_channels entries of cfg->freqs */
+} vdl2gpu_receiver;
+int vdl2gpu_create_receivers(const vdl2gpu_config *cfg, const vdl2gpu_receiver *rx, uint32_t n_rx, vdl2gpu_ctx **out);
 int vdl2gpu_destroy(vdl2gpu_ctx *ctx);
 const char *vdl2gpu_strerror(int code);
 const char *vdl2gpu_last_error(void);
