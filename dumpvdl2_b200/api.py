@@ -39,6 +39,10 @@ class _Receiver(C.Structure):
     _fields_ = [("centerfreq", C.c_uint32), ("n_channels", C.c_uint32)]
 
 
+class _ReceiverEx(C.Structure):
+    _fields_ = [("centerfreq", C.c_uint32), ("n_channels", C.c_uint32), ("oversample", C.c_uint32), ("sample_fmt", C.c_uint32)]
+
+
 class _Frame(C.Structure):
     _fields_ = [("channel", C.c_uint32), ("freq", C.c_uint32), ("burst_seq", C.c_uint32), ("idx", C.c_int32),
                 ("data", C.POINTER(C.c_uint8)), ("len", C.c_uint32), ("synd_weight", C.c_uint32),
@@ -75,6 +79,9 @@ def load_library():
     L = C.CDLL(LIB_PATH)
     L.vdl2gpu_create.argtypes = [C.POINTER(_Config), C.POINTER(C.c_void_p)]
     L.vdl2gpu_create_receivers.argtypes = [C.POINTER(_Config), C.POINTER(_Receiver), C.c_uint32, C.POINTER(C.c_void_p)]
+    L.vdl2gpu_create_mixed_receivers.argtypes = [C.POINTER(_Config), C.POINTER(_ReceiverEx), C.c_uint32, C.POINTER(C.c_void_p)]
+    L.vdl2gpu_submit_span.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.vdl2gpu_submit_span_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
     L.vdl2gpu_destroy.argtypes = [C.c_void_p]
     L.vdl2gpu_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
@@ -389,3 +396,73 @@ class Vdl2Receivers(Vdl2Channels):
         parts = [np.ascontiguousarray(b).view(np.uint8).reshape(-1) for b in bufs]
         for off in range(0, parts[0].size, chunk_bytes):
             self.submit([p[off:off + chunk_bytes] for p in parts])
+
+
+class Vdl2MixedReceivers(Vdl2Receivers):
+    """Receivers of different sample rates and sample formats on one H100 (e.g. RTL-SDR dongles, cu8 at 1.05 Msps, next to
+    SDRplay devices, cs16 at 2.1 Msps); every receiver decodes exactly as one reference process at its own rate, tuned to
+    its own centre, would.  The receivers advance in lock step in decimated samples (105000 per second for every rate):
+    submit_span() takes one buffer per receiver, receiver r's holding n_dec x oversample_r complex samples in its own
+    format.  Listing the receivers grouped by rate keeps every K1 warp on one rate (faster than interleaved rates)."""
+
+    def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4):
+        """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16))"""
+        self.L = load_library()
+        rxs = [(int(cf), [int(f) for f in fr], int(os_), int(fmt)) for cf, fr, os_, fmt in receivers]
+        self.receivers = [(cf, fr) for cf, fr, _, _ in rxs]
+        self.oversample = [os_ for _, _, os_, _ in rxs]
+        self.formats = [fmt for _, _, _, fmt in rxs]
+        self.bytes_per_dec = [os_ * (4 if fmt == FMT_S16 else 2) for _, _, os_, fmt in rxs]
+        self.n_receivers = self.n_streams = len(rxs)
+        self.freqs = np.ascontiguousarray([f for _, fr in self.receivers for f in fr], dtype=np.uint32)
+        self.n_channels = int(self.freqs.size)
+        self._first = np.concatenate([[0], np.cumsum([len(fr) for _, fr in self.receivers], dtype=np.int64)]).astype(np.int64)
+        self.sample_fmt = None
+        rx = (_ReceiverEx * max(self.n_receivers, 1))()
+        for r, (cf, fr, os_, fmt) in enumerate(rxs):
+            rx[r].centerfreq, rx[r].n_channels, rx[r].oversample, rx[r].sample_fmt = cf, len(fr), os_, fmt
+        cfg = _Config()                              # sample_rate, oversample, sample_fmt and centerfreq stay 0: per receiver
+        cfg.n_channels = self.n_channels
+        cfg.freqs = self.freqs.ctypes.data_as(C.POINTER(C.c_uint32))
+        cfg.max_ppm, cfg.max_chunk_bytes, cfg.device, cfg.flags, cfg.n_inflight = max_ppm, max_chunk_bytes, device, flags, n_inflight
+        cfg.n_streams = self.n_receivers
+        self.h = C.c_void_p()
+        _check(self.L, self.L.vdl2gpu_create_mixed_receivers(C.byref(cfg), rx, self.n_receivers, C.byref(self.h)),
+               "vdl2gpu_create_mixed_receivers")
+        self._frames = []
+        self._cb = _FRAME_CB(self._on_frame)
+
+    def _submit(self, buf, fmt):
+        raise Vdl2GpuError("a mixed-receivers context takes spans of decimated samples: use submit_span / submit_span_device")
+
+    def submit(self, bufs):
+        return self._submit(bufs, None)
+
+    def submit_device(self, dev_ptr, nbytes, producer_stream=0):
+        return self._submit(None, None)
+
+    def submit_span(self, bufs):
+        """one buffer per receiver; receiver r's holds n_dec x oversample_r complex samples in its own format"""
+        if len(bufs) != self.n_receivers:
+            raise Vdl2GpuError(f"{len(bufs)} buffers for {self.n_receivers} receivers")
+        parts = [np.ascontiguousarray(b).view(np.uint8).reshape(-1) for b in bufs]
+        n_dec = parts[0].size // self.bytes_per_dec[0]
+        for r, p in enumerate(parts):
+            if p.size != n_dec * self.bytes_per_dec[r]:
+                raise Vdl2GpuError(f"receiver {r}: {p.size} bytes, not {n_dec} decimated samples x {self.bytes_per_dec[r]} bytes")
+        buf = np.concatenate(parts)
+        _check(self.L, self.L.vdl2gpu_submit_span(self.h, buf.ctypes.data, n_dec), "vdl2gpu_submit_span")
+
+    def submit_span_device(self, dev_ptr, n_dec, producer_stream=0):
+        """the receivers' buffers back to back in device memory (receiver 0 first), n_dec decimated samples each"""
+        _check(self.L, self.L.vdl2gpu_submit_span_device(self.h, C.c_void_p(dev_ptr), n_dec, C.c_void_p(producer_stream)),
+               "vdl2gpu_submit_span_device")
+
+    def process_chunked(self, bufs, n_dec):
+        """each receiver's whole stream (the same duration for all), submitted n_dec decimated samples at a time; the last
+        span may be shorter"""
+        parts = [np.ascontiguousarray(b).view(np.uint8).reshape(-1) for b in bufs]
+        total = parts[0].size // self.bytes_per_dec[0]
+        for d0 in range(0, total, n_dec):
+            d1 = min(total, d0 + n_dec)
+            self.submit_span([p[d0 * w:d1 * w] for p, w in zip(parts, self.bytes_per_dec)])

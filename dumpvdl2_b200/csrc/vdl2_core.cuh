@@ -1191,4 +1191,49 @@ VDL2_HD uint32_t vdl2_rx_tile_samples(uint32_t G, uint32_t oversample) {
 	return (r - 2u) / step * step;
 }
 
+/* ------------------------------------------------------------------------------------------------
+ * Mixed-rate receivers (vdl2gpu_create_mixed_receivers): every receiver has its own oversample factor (10, 13 or 20) and
+ * sample format, and a span carries the same number n_dec of decimated samples for each of them
+ * ---------------------------------------------------------------------------------------------- */
+/* one receiver's input: oversample factor, sample format and the bytes that lie before its buffer in a span, per decimated
+ * sample of the span (receiver r's buffer starts n_dec * off_per_dec bytes in) */
+typedef struct {
+	uint64_t off_per_dec;
+	uint32_t oversample, fmt;
+} vdl2_rx_input;
+
+/* rate class of an oversample factor (index into the per-class filter taps); 10, 13 and 20 only */
+VDL2_HD uint32_t vdl2_rx_class(uint32_t oversample) { return oversample == 10u ? 0u : oversample == 13u ? 1u : 2u; }
+
+/* fills rx[r].off_per_dec = sum over q < r of os_q x bytes per complex sample of q; returns the bytes of one decimated
+ * sample of every receiver, i.e. a span of n_dec is n_dec times that long */
+VDL2_HD uint64_t vdl2_rx_span_layout(const uint32_t *oversample, const uint32_t *fmt, uint32_t n_rx, vdl2_rx_input *rx) {
+	uint64_t off = 0;
+	for(uint32_t r = 0; r < n_rx; r++) {
+		rx[r].off_per_dec = off;
+		rx[r].oversample = oversample[r];
+		rx[r].fmt = fmt[r];
+		off += (uint64_t)oversample[r] * (fmt[r] == 1u ? 4u : 2u);
+	}
+	return off;
+}
+
+/* byte offset of receiver r's buffer in a span of n_dec decimated samples (64 bits: 65535 cs16 receivers at oversample 20
+ * pass 4 GiB within a span of 55 decimated samples) */
+VDL2_HD uint64_t vdl2_rx_span_offset(const vdl2_rx_input *rx, uint32_t r, uint32_t n_dec) { return (uint64_t)n_dec * rx[r].off_per_dec; }
+
+/* Decimation groups per tile of the mixed K1 for blocks of up to G receivers whose largest oversample factor is os_max:
+ * row r of a tile stages TG x os_r samples into a row of vdl2_rx_tile_stride(TG x os_max) elements.  TG is even, so every
+ * row start and every copy size is a multiple of 16 bytes whatever the factors.  The largest even TG that keeps
+ * vdl2_rx_k1_smem_bytes within VDL2_RX_K1_SMEM_BUDGET; never below 2: with os_max 20 and 100 or more receivers in one
+ * block not even two groups fit, and the block then takes vdl2_rx_k1_smem_bytes(G, 40) > budget (at most
+ * VDL2_RX_MIXED_SMEM_MAX) - correct, but its K1 block no longer shares an SM with a K2 block. */
+VDL2_HD uint32_t vdl2_rx_mixed_tile_groups(uint32_t G, uint32_t os_max) {
+	if(G == 0) G = 1;
+	uint32_t tg = 2;
+	while(vdl2_rx_k1_smem_bytes(G, (tg + 2u) * os_max) <= VDL2_RX_K1_SMEM_BUDGET) tg += 2u;
+	return tg;
+}
+#define VDL2_RX_MIXED_SMEM_MAX (2u * VDL2_RX_K1_BLOCK * (40u + 10u) * 8u + VDL2_RX_K1_LUT_BYTES + 16u)   /* G = 128, TG = 2, os 20 */
+
 #endif

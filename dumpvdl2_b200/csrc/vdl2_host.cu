@@ -89,6 +89,16 @@ struct vdl2gpu_ctx {
 	bool receivers = false;                             /* vdl2gpu_create_receivers: n_streams receivers, each with its own centre and channels */
 	uint32_t *d_slot_rx = nullptr, *d_block_rx = nullptr;   /* receivers: vdl2_rx_layout tables (fixed at create) */
 	uint32_t rx_tile = 0, rx_max = 0;                   /* receivers: samples per staged tile, most receivers of one K1 block */
+	/* mixed-rate receivers (vdl2gpu_create_mixed_receivers): every receiver has its own oversample factor and format, and
+	 * the chain counts DECIMATED samples (n_pairs of a chunk = n_dec of a span, decimation counter always 0); rx_tile is
+	 * then the decimation groups of a staged tile */
+	bool mixed = false;
+	std::vector<vdl2_rx_input> rx_in;                   /* per receiver: oversample, format, byte offset per decimated sample */
+	vdl2_rx_input *d_rx_in = nullptr;
+	uint8_t *d_slot_cls = nullptr;                      /* slot -> rate class (vdl2_rx_class) of its receiver */
+	uint64_t span_bytes_per_dec = 0, span_pairs_per_dec = 0;   /* sums over the receivers of os x bytes per sample, of os */
+	uint32_t max_span = 0, rx_os_max = 0, cls_mask = 0;  /* largest n_dec of a span; largest oversample; rate classes present */
+	float cls_taps[3][5] = {};                          /* {a0, a1, a2, b1, b2} per rate class (10, 13, 20) */
 	uint32_t raw_bytes = 0;                             /* size of each slot's raw staging buffers (allocated on the first host submit) */
 	int k1_variant = 2, k2_variant = 5, k2a_mode = 1;   /* A/B knobs (VDL2GPU_K1_VARIANT, VDL2GPU_K2_VARIANT, VDL2GPU_K2A), read at create */
 	bool use_graphs = true;
@@ -133,8 +143,8 @@ static uint32_t dphi_for(uint32_t centerfreq, uint32_t freq, uint32_t rate) {   
 	return (uint32_t)(int)(((float)centerfreq - (float)freq) / (float)rate * 256.0f * 65536.0f);
 }
 
-static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, uint32_t n_ch, uint32_t n_chp,
-		uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2);
+static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
+		uint32_t n_chp, uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2);
 /* channel -> slot: the first full_warps warps hold `lanes` channels each, the others lanes - 1 */
 static inline uint32_t slot_of(uint32_t ch, uint32_t lanes, uint32_t full_warps) {
 	const uint32_t head = full_warps * lanes;
@@ -193,6 +203,7 @@ static int free_ctx(vdl2gpu_ctx *c) {
 	cudaFree(c->d_counters); cudaFree(c->d_ready); cudaFree(c->d_ring); cudaFree(c->d_pool); cudaFree(c->d_free);
 	cudaFree(c->d_ctl); cudaFree(c->d_events); cudaFree(c->d_block_trace);
 	cudaFree(c->d_slot_rx); cudaFree(c->d_block_rx);
+	cudaFree(c->d_rx_in); cudaFree(c->d_slot_cls);
 	if(c->ev_input_ready) cudaEventDestroy(c->ev_input_ready);
 	if(c->ev_input_consumed) cudaEventDestroy(c->ev_input_consumed);
 	if(c->ev_drain) cudaEventDestroy(c->ev_drain);
@@ -206,8 +217,10 @@ static int free_ctx(vdl2gpu_ctx *c) {
 	return VDL2GPU_OK;
 }
 
-/* rx / n_rx: the receivers of a multi-receiver context (vdl2gpu_create_receivers, validated there), NULL / 0 otherwise */
-static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_receiver *rx = nullptr, uint32_t n_rx = 0) {
+/* rx / n_rx: the receivers of a multi-receiver context (vdl2gpu_create_receivers, validated there), NULL / 0 otherwise;
+ * rx_ex: the same receivers with their oversample factors and formats (vdl2gpu_create_mixed_receivers), NULL otherwise */
+static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_receiver *rx = nullptr, uint32_t n_rx = 0,
+		const vdl2gpu_receiver_ex *rx_ex = nullptr) {
 	int ndev = 0;
 	cudaError_t e = cudaGetDeviceCount(&ndev);
 	if(e != cudaSuccess || ndev == 0) {
@@ -227,6 +240,7 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	KL(vdl2_kernels_init_device(c->device));             /* per device: function attributes do not carry over */
 	c->cfg = *cfg;
 	c->receivers = rx != nullptr;
+	c->mixed = rx_ex != nullptr;
 	c->n_streams = c->receivers ? n_rx : cfg->n_streams ? cfg->n_streams : 1u;
 	c->cfg.n_streams = c->n_streams;
 	c->lane_streams = !c->receivers && c->n_streams > 1 && c->n_streams == cfg->n_channels;     /* one stream per channel */
@@ -287,9 +301,26 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	}
 	const uint32_t max_bytes = cfg->max_chunk_bytes ? cfg->max_chunk_bytes : (1u << 20);
 	c->cfg.max_chunk_bytes = max_bytes;
-	c->max_pairs = max_bytes / (cfg->sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
-	if(c->receivers) c->max_pairs = (c->max_pairs + 1u) & ~1u;     /* even row stride: every receiver row of the plane starts 16-byte aligned */
-	c->max_dec = c->max_pairs / cfg->oversample + 2;
+	if(c->mixed) {
+		/* the largest span: every receiver's buffer within max_chunk_bytes; the plane's row stride holds the longest row */
+		uint32_t bpd_max = 0;
+		for(uint32_t r = 0; r < n_rx; r++) {
+			bpd_max = std::max(bpd_max, rx_ex[r].oversample * (rx_ex[r].sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u));
+			c->rx_os_max = std::max(c->rx_os_max, rx_ex[r].oversample);
+		}
+		c->max_span = max_bytes / bpd_max;
+		if(c->max_span == 0) {
+			snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_create_mixed_receivers: max_chunk_bytes (%u) holds less than one decimated sample of a receiver (%u bytes)",
+					max_bytes, bpd_max);
+			return VDL2GPU_EINVAL;
+		}
+		c->max_pairs = (c->max_span * c->rx_os_max + 1u) & ~1u;       /* even row stride: every row of the plane starts 16-byte aligned */
+		c->max_dec = c->max_span + 2;
+	} else {
+		c->max_pairs = max_bytes / (cfg->sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
+		if(c->receivers) c->max_pairs = (c->max_pairs + 1u) & ~1u;     /* even row stride: every receiver row of the plane starts 16-byte aligned */
+		c->max_dec = c->max_pairs / cfg->oversample + 2;
+	}
 	if((uint64_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp >= (1ull << 32)) {
 		snprintf(g_last_error, sizeof(g_last_error), "%u channels x %u decimated samples per chunk exceed the 32-bit element index of the kernels; "
 				"use a smaller max_chunk_bytes or shard the channels", c->n_ch, c->max_dec);
@@ -300,7 +331,8 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	const uint32_t n_inflight = cfg->n_inflight ? cfg->n_inflight : 4u;
 	c->cfg.n_inflight = n_inflight;
 	c->event_cap = (cfg->flags & VDL2GPU_FLAG_TRACE) ? (1u << 20) : 1u;
-	make_tables(c->tab, cfg->sample_rate);
+	/* (mixed receivers: the rate only enters the filter taps of these tables, which the mixed K1 takes per rate class) */
+	make_tables(c->tab, c->mixed ? (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * c->rx_os_max : cfg->sample_rate);
 	memset(&c->stats, 0, sizeof(c->stats));
 
 	/* equal (default) priorities: raising either stage's priority slowed the pair down (tools/probe_overlap.py) */
@@ -351,24 +383,50 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	CU(cudaMemset(c->d_ring, 0, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
 	CU(cudaMemset(c->d_pool, 0, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
 
-	std::vector<uint32_t> k1, k2, centres;
+	std::vector<uint32_t> k1, k2, centres, rates;
 	if(c->receivers) {
 		/* every channel mixes against its own receiver's centre (src/demod.c:385); the slot -> receiver tables K1 stages by */
 		std::vector<uint32_t> rx_first(n_rx + 1, 0);
 		for(uint32_t r = 0; r < n_rx; r++) {
 			rx_first[r + 1] = rx_first[r] + rx[r].n_channels;
 			centres.insert(centres.end(), rx[r].n_channels, rx[r].centerfreq);
+			if(c->mixed) rates.insert(rates.end(), rx[r].n_channels, (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * rx_ex[r].oversample);
 		}
 		const uint32_t n_blocks = (c->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
 		std::vector<uint32_t> slot_rx((size_t)n_blocks * VDL2_RX_K1_BLOCK), block_rx(2 * (size_t)n_blocks);
 		c->rx_max = vdl2_rx_layout(n_blocks, c->lanes, c->full_warps, c->n_ch, rx_first.data(), n_rx, slot_rx.data(), block_rx.data());
-		c->rx_tile = vdl2_rx_tile_samples(c->rx_max, cfg->oversample);
+		c->rx_tile = c->mixed ? vdl2_rx_mixed_tile_groups(c->rx_max, c->rx_os_max) : vdl2_rx_tile_samples(c->rx_max, cfg->oversample);
 		CU(cudaMalloc(&c->d_slot_rx, slot_rx.size() * 4));
 		CU(cudaMalloc(&c->d_block_rx, block_rx.size() * 4));
 		CU(cudaMemcpy(c->d_slot_rx, slot_rx.data(), slot_rx.size() * 4, cudaMemcpyHostToDevice));
 		CU(cudaMemcpy(c->d_block_rx, block_rx.data(), block_rx.size() * 4, cudaMemcpyHostToDevice));
+		if(c->mixed) {
+			/* per receiver: oversample, format, place in a span; per slot: rate class; per class: the filter taps of
+			 * input_lpf_init(105000 x os) (src/demod.c:367-370) */
+			std::vector<uint32_t> os(n_rx), fmt(n_rx);
+			for(uint32_t r = 0; r < n_rx; r++) { os[r] = rx_ex[r].oversample; fmt[r] = rx_ex[r].sample_fmt; }
+			c->rx_in.resize(n_rx);
+			c->span_bytes_per_dec = vdl2_rx_span_layout(os.data(), fmt.data(), n_rx, c->rx_in.data());
+			for(uint32_t r = 0; r < n_rx; r++) {
+				c->span_pairs_per_dec += os[r];
+				c->cls_mask |= 1u << vdl2_rx_class(os[r]);
+			}
+			static const uint32_t class_os[3] = { 10, 13, 20 };
+			for(int k = 0; k < 3; k++) {
+				float A[3], B[3];
+				make_lpf((uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * class_os[k], A, B);
+				c->cls_taps[k][0] = A[0]; c->cls_taps[k][1] = A[1]; c->cls_taps[k][2] = A[2]; c->cls_taps[k][3] = B[1]; c->cls_taps[k][4] = B[2];
+			}
+			std::vector<uint8_t> slot_cls(slot_rx.size());
+			for(size_t s = 0; s < slot_rx.size(); s++) slot_cls[s] = (uint8_t)vdl2_rx_class(os[slot_rx[s]]);
+			CU(cudaMalloc(&c->d_rx_in, c->rx_in.size() * sizeof(vdl2_rx_input)));
+			CU(cudaMalloc(&c->d_slot_cls, slot_cls.size()));
+			CU(cudaMemcpy(c->d_rx_in, c->rx_in.data(), c->rx_in.size() * sizeof(vdl2_rx_input), cudaMemcpyHostToDevice));
+			CU(cudaMemcpy(c->d_slot_cls, slot_cls.data(), slot_cls.size(), cudaMemcpyHostToDevice));
+		}
 	}
-	initial_state(c->cfg, c->freqs.data(), c->receivers ? centres.data() : nullptr, c->n_ch, c->n_chp, c->lanes, c->full_warps, k1, k2);
+	initial_state(c->cfg, c->freqs.data(), c->receivers ? centres.data() : nullptr, c->mixed ? rates.data() : nullptr, c->n_ch, c->n_chp,
+			c->lanes, c->full_warps, k1, k2);
 	CU(cudaMemcpy(c->d_k1, k1.data(), k1.size() * 4, cudaMemcpyHostToDevice));
 	CU(cudaMemcpy(c->d_k2, k2.data(), k2.size() * 4, cudaMemcpyHostToDevice));
 	std::vector<int32_t> fl(c->n_slots);
@@ -431,6 +489,43 @@ extern "C" int vdl2gpu_create_receivers(const vdl2gpu_config *cfg, const vdl2gpu
 	}
 	vdl2gpu_ctx *c = new vdl2gpu_ctx();
 	int rc = create_impl(cfg, c, rx, n_rx);
+	if(rc != VDL2GPU_OK) { free_ctx(c); *out = nullptr; return rc; }
+	*out = c;
+	return VDL2GPU_OK;
+}
+
+extern "C" int vdl2gpu_create_mixed_receivers(const vdl2gpu_config *cfg, const vdl2gpu_receiver_ex *rx, uint32_t n_rx, vdl2gpu_ctx **out) {
+	const char *why = nullptr;
+	char buf[160];
+	uint64_t sum = 0;
+	if(!cfg || !out || !cfg->freqs || cfg->n_channels == 0) why = "bad vdl2gpu_config (no channels)";
+	else if(cfg->sample_rate || cfg->oversample || cfg->sample_fmt || cfg->centerfreq)
+		why = "cfg->sample_rate, oversample, sample_fmt and centerfreq must be 0 (they are per receiver)";
+	else if(!rx || n_rx == 0) why = "no receivers";
+	else if(n_rx > 65535u) why = "more than 65535 receivers (one K0 grid row each)";
+	else if(cfg->n_streams != 0 && cfg->n_streams != n_rx) why = "n_streams must be 0 or the number of receivers";
+	else if(cfg->flags & VDL2GPU_FLAG_K1_SCALAR) why = "VDL2GPU_FLAG_K1_SCALAR is not available with receivers";
+	else {
+		for(uint32_t r = 0; r < n_rx && !why; r++) {
+			if(rx[r].n_channels == 0) { snprintf(buf, sizeof(buf), "receiver %u has no channels", r); why = buf; }
+			else if(rx[r].oversample != 10 && rx[r].oversample != 13 && rx[r].oversample != 20) {
+				snprintf(buf, sizeof(buf), "receiver %u: oversample %u (10, 13 or 20 only)", r, rx[r].oversample); why = buf;
+			} else if(rx[r].sample_fmt > 1) {
+				snprintf(buf, sizeof(buf), "receiver %u: sample format %u (VDL2GPU_FMT_U8 or VDL2GPU_FMT_S16_LE only)", r, rx[r].sample_fmt); why = buf;
+			}
+			sum += rx[r].n_channels;
+		}
+		if(!why && sum != cfg->n_channels) why = "the receivers' channel counts do not add up to n_channels";
+	}
+	if(why) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_create_mixed_receivers: %s", why);
+		if(out) *out = nullptr;
+		return VDL2GPU_EINVAL;
+	}
+	std::vector<vdl2gpu_receiver> base(n_rx);
+	for(uint32_t r = 0; r < n_rx; r++) { base[r].centerfreq = rx[r].centerfreq; base[r].n_channels = rx[r].n_channels; }
+	vdl2gpu_ctx *c = new vdl2gpu_ctx();
+	int rc = create_impl(cfg, c, base.data(), n_rx, rx);
 	if(rc != VDL2GPU_OK) { free_ctx(c); *out = nullptr; return rc; }
 	*out = c;
 	return VDL2GPU_OK;
@@ -533,7 +628,8 @@ static void harvest(vdl2gpu_ctx *c, chunk_slot &s) {
 	const uint32_t used = std::min(h->bytes_used, c->out_cap);
 	c->blobs.emplace_back(s.h_out, s.h_out + sizeof(vdl2_out_header) + used);
 	const uint32_t blob_id = (uint32_t)c->blobs.size() - 1;
-	const double rate = (double)c->cfg.sample_rate / (double)c->cfg.oversample;     /* decimated samples per second */
+	/* decimated samples per second (105000 for every receiver of a mixed context, whose config carries no rate) */
+	const double rate = c->mixed ? (double)VDL2_SYMBOL_RATE * VDL2_SPS : (double)c->cfg.sample_rate / (double)c->cfg.oversample;
 	parse_region(c->blobs.back().data(), c->out_cap, rate, s.arrival, s.dec_base + s.n_dec, blob_id, c->pending, c->stats);
 	c->stats.chunks_completed++;
 	s.busy = false;
@@ -603,6 +699,8 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	p1.trace_blocks = c->d_block_trace; p2.trace_blocks = c->d_block_trace;
 	p1.ch_per_stream = c->ch_per_stream; p1.stream_stride = c->lane_streams ? c->n_chp : c->max_pairs; p1.ca = ca;
 	p1.slot_rx = c->d_slot_rx; p1.block_rx = c->d_block_rx; p1.rx_tile = c->rx_tile; p1.rx_max = c->rx_max;
+	p1.rx_in = c->d_rx_in; p1.slot_cls = c->d_slot_cls; p1.cls_mask = c->cls_mask; p1.rx_os_max = c->rx_os_max;
+	memcpy(p1.cls_taps, c->cls_taps, sizeof(p1.cls_taps));
 	p1.phase = c->fuse_phase ? c->d_phase2[pb] : nullptr; p1.phase_prev = c->d_phase2[pb ^ 1]; p1.prev_n_dec = prev_n_dec;
 	/* the default walk (variant 5) computes the four magnitudes a block needs from the staged samples: no magnitude plane */
 	const bool need_mag = (c->k2_variant & 0xFF) >= 0 && (c->k2_variant & 0xFF) <= 4;
@@ -637,12 +735,22 @@ static int capture_one(cudaStream_t st, cudaGraphExec_t *out, int (*body)(void *
 	return VDL2GPU_OK;
 }
 
+/* input samples per decimated sample as the chain counts them: a mixed-rate context counts decimated samples directly */
+static inline uint32_t chain_os(const vdl2gpu_ctx *c) { return c->mixed ? 1u : c->cfg.oversample; }
+
+/* mixed-rate receivers: K0 of a span of n_dec decimated samples into the sample plane (ca: graph replay) */
+static int launch_k0_mixed(vdl2gpu_ctx *c, const void *d_raw, uint32_t n_dec, const vdl2_chunk_args *ca) {
+	KL(vdl2_launch_k0_mixed(d_raw, n_dec, c->d_rx_in, c->n_streams, c->rx_os_max, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples),
+			c->max_pairs, ca, c->stream));
+	return VDL2GPU_OK;
+}
+
 struct capture_env { vdl2gpu_ctx *c; chunk_slot *s; uint64_t seq; uint32_t n_pairs; uint32_t k0_fmt; };
 #define CAPTURE_PARAMS \
 	capture_env *e = static_cast<capture_env *>(a); \
 	vdl2gpu_ctx *c = e->c; \
 	vdl2_k1_params p1; vdl2_k2a_params pa; vdl2_k2_params p2; vdl2_k3_params p3; \
-	const uint32_t os = c->cfg.oversample; \
+	const uint32_t os = chain_os(c); \
 	fill_params(c, *e->s, e->seq, e->n_pairs, 0, (os - 1 + e->n_pairs) / os, 0, 0, e->s->d_args, p1, pa, p2, p3)
 
 static int body_front(void *a) {
@@ -650,7 +758,8 @@ static int body_front(void *a) {
 	(void)pa; (void)p2; (void)p3;
 	CU(cudaMemcpyAsync(e->s->d_args, e->s->h_args, sizeof(vdl2_chunk_args), cudaMemcpyHostToDevice, c->stream));
 	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
-	if(c->lane_streams) KL(vdl2_launch_k0_lanes(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
+	if(c->mixed) { int rc = launch_k0_mixed(c, nullptr, e->n_pairs, e->s->d_args); if(rc) return rc; }
+	else if(c->lane_streams) KL(vdl2_launch_k0_lanes(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 			e->n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, e->s->d_args, c->stream));
 	else KL(vdl2_launch_k0(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 			e->n_pairs * bpp, c->max_pairs, e->s->d_args, c->stream));
@@ -685,8 +794,9 @@ static int ensure_graphs(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n
 	return rc;
 }
 
+/* n_pairs: complex samples per stream; in a mixed-rate context, decimated samples per receiver (the span's n_dec) */
 static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t n_pairs, uint32_t k0_fmt = 0xFFFFFFFFu) {
-	const uint32_t os = c->cfg.oversample;
+	const uint32_t os = chain_os(c);
 	const bool planar = k0_fmt != 0xFFFFFFFFu;
 	if(!planar) k0_fmt = c->cfg.sample_fmt;
 	s.first_pair = c->total_pairs;
@@ -725,7 +835,8 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	if(graph) {
 		CU(cudaGraphLaunch(s.g_front[gk], c->stream));
 	} else {
-		if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
+		if(c->mixed) { int rc = launch_k0_mixed(c, d_raw, n_pairs, nullptr); if(rc) return rc; }
+		else if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 				n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, nullptr, c->stream));
 		else KL(vdl2_launch_k0(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 				n_pairs * bpp, c->max_pairs, nullptr, c->stream));
@@ -772,14 +883,21 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	c->total_dec += s.n_dec;
 	c->last_n_dec = s.n_dec;
 	c->stats.chunks_submitted++;
-	c->stats.iq_samples += n_pairs;
+	c->stats.iq_samples += c->mixed ? (uint64_t)n_pairs * c->span_pairs_per_dec : n_pairs;
 	c->stats.dec_samples += s.n_dec;
 	c->stats.kernel_launches += (n_pairs ? 2 : 0) + (c->fuse_phase ? 0 : 1) + (s.n_dec ? 1 : 0) + 2;
 	return VDL2GPU_OK;
 }
 
+/* the byte-length submits have no meaning for receivers of different rates: their buffers differ in length */
+static int refuse_mixed(const char *what) {
+	snprintf(g_last_error, sizeof(g_last_error), "%s: a mixed-receivers context takes spans of decimated samples (vdl2gpu_submit_span, vdl2gpu_submit_span_device)", what);
+	return VDL2GPU_EINVAL;
+}
+
 extern "C" int vdl2gpu_submit(vdl2gpu_ctx *c, const void *iq, uint32_t len) {
 	if(!c || (!iq && len)) return VDL2GPU_EINVAL;
+	if(c->mixed) return refuse_mixed("vdl2gpu_submit");
 	if(len == 0) return VDL2GPU_OK;                                   /* src/demod.c:341,358 */
 	if(len > c->cfg.max_chunk_bytes) return VDL2GPU_ETOOBIG;
 	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
@@ -802,6 +920,7 @@ extern "C" int vdl2gpu_submit(vdl2gpu_ctx *c, const void *iq, uint32_t len) {
 
 extern "C" int vdl2gpu_submit_planar_s16(vdl2gpu_ctx *c, const int16_t *xi, const int16_t *xq, uint32_t n_pairs) {
 	if(!c || ((!xi || !xq) && n_pairs)) return VDL2GPU_EINVAL;
+	if(c->mixed) return refuse_mixed("vdl2gpu_submit_planar_s16");
 	if(c->cfg.sample_fmt != VDL2GPU_FMT_S16_LE || c->n_streams != 1 || c->receivers) return VDL2GPU_EINVAL;
 	if(n_pairs == 0) return VDL2GPU_OK;
 	if((uint64_t)n_pairs * 4u > c->cfg.max_chunk_bytes) return VDL2GPU_ETOOBIG;
@@ -861,6 +980,7 @@ extern "C" int vdl2gpu_serialize_raw_frame(const vdl2gpu_frame *f, const char *s
 
 extern "C" int vdl2gpu_submit_device(vdl2gpu_ctx *c, const void *dev_iq, uint32_t len, void *producer_stream) {
 	if(!c || (!dev_iq && len)) return VDL2GPU_EINVAL;
+	if(c->mixed) return refuse_mixed("vdl2gpu_submit_device");
 	if(len == 0) return VDL2GPU_OK;
 	if(len > c->cfg.max_chunk_bytes) return VDL2GPU_ETOOBIG;
 	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
@@ -874,6 +994,61 @@ extern "C" int vdl2gpu_submit_device(vdl2gpu_ctx *c, const void *dev_iq, uint32_
 	CU(cudaEventRecord(c->ev_input_ready, (cudaStream_t)producer_stream));
 	CU(cudaStreamWaitEvent(c->stream, c->ev_input_ready, 0));
 	return run_chain(c, *s, dev_iq, n_pairs);
+}
+
+/* spans: the common checks of the two submits.  Returns 1 for a mixed-rate context (go on), 0 after forwarding a uniform
+ * receivers context's span as `*len` bytes per receiver (the caller submits it), or a negative error. */
+static int span_check(vdl2gpu_ctx *c, const void *iq, uint32_t n_dec, const char *what, uint32_t *len) {
+	if(!c || (!iq && n_dec)) return VDL2GPU_EINVAL;
+	if(!c->receivers) {
+		snprintf(g_last_error, sizeof(g_last_error), "%s: spans need a receivers context (vdl2gpu_create_mixed_receivers or vdl2gpu_create_receivers)", what);
+		return VDL2GPU_EINVAL;
+	}
+	if(c->mixed) {
+		if(n_dec > c->max_span) {
+			snprintf(g_last_error, sizeof(g_last_error), "%s: %u decimated samples per span, at most %u fit max_chunk_bytes", what, n_dec, c->max_span);
+			return VDL2GPU_ETOOBIG;
+		}
+		return 1;
+	}
+	const uint64_t bytes = (uint64_t)n_dec * c->cfg.oversample * (c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
+	if(bytes > c->cfg.max_chunk_bytes) return VDL2GPU_ETOOBIG;
+	*len = (uint32_t)bytes;
+	return 0;
+}
+
+extern "C" int vdl2gpu_submit_span(vdl2gpu_ctx *c, const void *iq, uint32_t n_dec) {
+	uint32_t len = 0;
+	int rc = span_check(c, iq, n_dec, "vdl2gpu_submit_span", &len);
+	if(rc < 0) return rc;
+	if(rc == 0) return vdl2gpu_submit(c, iq, len);
+	if(n_dec == 0) return VDL2GPU_OK;
+	CU(cudaSetDevice(c->device));
+	chunk_slot *s;
+	rc = acquire_slot(c, &s);
+	if(rc) return rc;
+	rc = ensure_raw(c, *s);
+	if(rc) return rc;
+	/* n_dec x span_bytes_per_dec <= max_chunk_bytes x n_rx, the size of the staging buffers */
+	const size_t bytes = (size_t)n_dec * c->span_bytes_per_dec;
+	memcpy(s->h_raw, iq, bytes);
+	CU(cudaMemcpyAsync(s->d_raw, s->h_raw, bytes, cudaMemcpyHostToDevice, c->stream));
+	return run_chain(c, *s, s->d_raw, n_dec);
+}
+
+extern "C" int vdl2gpu_submit_span_device(vdl2gpu_ctx *c, const void *dev_iq, uint32_t n_dec, void *producer_stream) {
+	uint32_t len = 0;
+	int rc = span_check(c, dev_iq, n_dec, "vdl2gpu_submit_span_device", &len);
+	if(rc < 0) return rc;
+	if(rc == 0) return vdl2gpu_submit_device(c, dev_iq, len, producer_stream);
+	if(n_dec == 0) return VDL2GPU_OK;
+	CU(cudaSetDevice(c->device));
+	chunk_slot *s;
+	rc = acquire_slot(c, &s);
+	if(rc) return rc;
+	CU(cudaEventRecord(c->ev_input_ready, (cudaStream_t)producer_stream));
+	CU(cudaStreamWaitEvent(c->stream, c->ev_input_ready, 0));
+	return run_chain(c, *s, dev_iq, n_dec);
 }
 
 extern "C" int vdl2gpu_wait_input_consumed(vdl2gpu_ctx *c, void *stream) {
@@ -967,6 +1142,10 @@ extern "C" int vdl2gpu_get_channel_counters(vdl2gpu_ctx *c, uint64_t *out, uint3
 extern "C" int vdl2gpu_get_tables(vdl2gpu_ctx *c, float levels[256], float sin_lut[257], float cos_lut[257],
 		float A[3], float B[3], float lr_X[16], float *lr_denom, float pr_phase[16]) {
 	if(!c) return VDL2GPU_EINVAL;
+	if(c->mixed) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_get_tables: a mixed-receivers context has no single sample rate (and filter)");
+		return VDL2GPU_EINVAL;
+	}
 	if(levels) memcpy(levels, c->tab.t.levels, sizeof(c->tab.t.levels));
 	if(sin_lut) memcpy(sin_lut, c->tab.sin_lut, sizeof(c->tab.sin_lut));
 	if(cos_lut) memcpy(cos_lut, c->tab.cos_lut, sizeof(c->tab.cos_lut));
@@ -1200,8 +1379,8 @@ extern "C" uint32_t vdl2gpu_stage_row_stride(uint32_t n_channels) { return (n_ch
 
 /* initial per-channel state: vdl2_channel_init + demod_reset (src/demod.c:205-220,379-392), process_samples locals
  * (src/demod.c:289-298); shared by the batch context and the stage stubs */
-static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, uint32_t n_ch, uint32_t n_chp,
-		uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2) {
+static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
+		uint32_t n_chp, uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2) {
 	k1.assign((size_t)K1_NFIELDS * n_chp, 0u); k2.assign((size_t)K2_NFIELDS * n_chp, 0u);
 	auto fbits = [](float f) { uint32_t u; memcpy(&u, &f, 4); return u; };
 	for(uint32_t chan = 0; chan < n_ch; chan++) {
@@ -1209,7 +1388,8 @@ static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, cons
 		/* a channel on the centre frequency skips the mixer in the reference (src/demod.c:312); with a zero
 		 * phase step the table gives cos = 1, sin = 0 and the products are exact, so no branch is needed */
 		const uint32_t centre = centres ? centres[chan] : cfg.centerfreq;     /* centres: per channel, multi-receiver context */
-		k1[(size_t)K1_DPHI * n_chp + ch] = (centre != freqs[chan]) ? dphi_for(centre, freqs[chan], cfg.sample_rate) : 0u;
+		const uint32_t rate = rates ? rates[chan] : cfg.sample_rate;          /* rates: per channel, mixed-rate receivers */
+		k1[(size_t)K1_DPHI * n_chp + ch] = (centre != freqs[chan]) ? dphi_for(centre, freqs[chan], rate) : 0u;
 		k2[(size_t)K2_MAG_NF * n_chp + ch] = fbits(2.0f);
 		k2[(size_t)K2_PHERR1 * n_chp + ch] = fbits(1000.f);
 		k2[(size_t)K2_PHERR2 * n_chp + ch] = fbits(1000.f);
@@ -1250,7 +1430,7 @@ extern "C" int vdl2gpu_stage_create(const vdl2gpu_config *cfg, uint32_t max_dec,
 	st->d_ready = reinterpret_cast<uint32_t *>(b + L.ready); st->d_ctl = reinterpret_cast<vdl2_queue_ctl *>(b + L.ctl);
 	st->d_events = b + L.events;
 	std::vector<uint32_t> k1, k2;
-	initial_state(st->cfg, st->freqs.data(), nullptr, st->n_ch, st->n_chp, 32u, 0xFFFFFFFFu, k1, k2);
+	initial_state(st->cfg, st->freqs.data(), nullptr, nullptr, st->n_ch, st->n_chp, 32u, 0xFFFFFFFFu, k1, k2);
 	std::vector<int32_t> fl(st->n_slots);
 	for(uint32_t i = 0; i < st->n_slots; i++) fl[i] = (int32_t)i;
 	vdl2_queue_ctl ctl;

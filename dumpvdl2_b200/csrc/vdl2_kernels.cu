@@ -95,6 +95,32 @@ __global__ void __launch_bounds__(1024) k0_convert_lanes(const uint8_t *__restri
 	if(i_out < n_pairs && s_out < out_stride) out[(size_t)i_out * out_stride + s_out] = tile[tx][ty];
 }
 
+/* K0 for mixed-rate receivers: grid row r converts receiver r's n_dec x os_r samples, in its own format, from its own
+ * place in the span (vdl2_rx_span_offset) into row r of the sample plane; the same arithmetic as k0_convert.  Rows of
+ * receivers with a smaller oversample factor than the largest leave their surplus threads idle. */
+__global__ void __launch_bounds__(256) k0_convert_mixed(const uint8_t *__restrict__ raw0, uint32_t n_dec_p, const vdl2_rx_input *__restrict__ rx,
+		const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride, const vdl2_chunk_args *__restrict__ ca) {
+	const uint32_t n_dec = ca ? ca->n_pairs : n_dec_p;
+	const vdl2_rx_input in = rx[blockIdx.y];
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= n_dec * in.oversample) return;
+	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec);
+	float re, im;
+	if(in.fmt == 0) {                                    /* src/demod.c:343-345, table from :349-354 */
+		uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
+		re = __ldg(&levels[v.x]);
+		im = __ldg(&levels[v.y]);
+	} else {                                             /* src/demod.c:361-363 */
+		/* a cs16 buffer after a cu8 one of odd n_dec x os starts 2 bytes off a 4-byte boundary: two 16-bit loads then */
+		short2 v;
+		if((reinterpret_cast<uintptr_t>(raw) & 3u) == 0) v = reinterpret_cast<const short2 *>(raw)[i];
+		else { const short *s = reinterpret_cast<const short *>(raw) + 2u * i; v = make_short2(s[0], s[1]); }
+		re = __fdiv_rn((float)v.x, 32768.0f);
+		im = __fdiv_rn((float)v.y, 32768.0f);
+	}
+	out0[(size_t)blockIdx.y * out_stride + i] = make_float2(re, im);
+}
+
 /* ------------------------------------------------------------------------------------------------
  * K1, plain per-sample form (reference for the pipelined kernel; selected by VDL2GPU_FLAG_K1_SCALAR
  * and for oversample values without a specialisation).
@@ -750,6 +776,138 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_groups(v
 }
 
 /* ------------------------------------------------------------------------------------------------
+ * K1, mixed-rate receivers (vdl2gpu_create_mixed_receivers): as k1_mix_iir_decimate_groups, but every receiver has its
+ * own oversample factor (10, 13 or 20) and filter taps.  A span holds n_dec decimated samples for every receiver, i.e.
+ * whole decimation groups: the decimation counter is always 0, and there is no head or tail sample loop.  Each tile covers
+ * the same TG = rx_tile decimation groups of every receiver of the block; row r stages TG x os_r samples into a row of
+ * vdl2_rx_tile_stride(TG x os_max) elements.  TG is even, so every row start in the plane and in shared memory and every
+ * copy size is a multiple of 16 bytes (no odd-phase shift); only a short last tile of an odd oversample factor ends on
+ * an odd sample, which the requesting lane copies by hand.  The tile loop (mbarrier waits, __syncthreads, the requests of
+ * warp 0) is uniform across the block; only the group body dispatches on the lane's factor.  Lanes of one warp that
+ * belong to receivers of different rates run the arms one after the other: correct, but listing the receivers grouped by
+ * rate keeps every warp (except at most two per rate boundary) on one arm.
+ * ---------------------------------------------------------------------------------------------- */
+/* ng decimation groups of one lane from its staged row: the software-pipelined group body of k1_mix_iir_decimate_groups,
+ * operation for operation (k1_packed_step's arithmetic, no contraction, the same rounding order) */
+template<int OS, bool SYM>
+__device__ __forceinline__ void k1m_groups(const float2 *s_row, uint32_t ng, float2 *dec, uint32_t n_chp, const float4 *s_lut,
+		uint32_t lane_bytes, uint32_t &phi, const uint32_t dphi, u64 &x1, u64 &x2, u64 &y1, u64 &y2, u64 &P1, u64 &P2,
+		const k1_packed_consts &c) {
+	constexpr int NLUT = 8, LA = 10, MA = 5;
+	for(uint32_t g = 0; g < ng; g++) {
+		const float2 *sp = &s_row[g * OS];
+		u64 y0 = 0;
+		float2 S[OS];
+		float4 E[OS];
+		float FR[OS];
+		u64 X0[OS];
+#pragma unroll
+		for(int k = -LA; k < OS; k++) {
+			const int kl = k + LA, km = k + MA;
+			if(kl < OS) {
+				const uint32_t ph = phi + (uint32_t)kl * dphi;
+				E[kl] = k1_lut_entry<NLUT>(s_lut, ph, lane_bytes);
+				FR[kl] = (float)(ph & 0xFFFFu);
+				S[kl] = sp[kl];
+			}
+			if(km >= 0 && km < OS) {
+				const u64 CS = f2_fma(f2_mul(f2_pack(E[km].z, E[km].w), f2_pack(FR[km], FR[km])), c.ONE, f2_pack(E[km].x, E[km].y));
+				X0[km] = k1_mix(S[km], CS, c);
+			}
+			if(k >= 0) {
+				const u64 x0 = X0[k];
+				u64 r;
+				if(SYM) {
+					const u64 P0 = f2_mul(c.A0, x0);
+					r = f2_fma(P0, c.ONE, f2_fma(P1, c.TWO, P2));
+					P2 = P1; P1 = P0;
+				} else {
+					const u64 t = f2_fma(f2_mul(c.A1, x1), c.ONE, f2_mul(c.A2, x2));
+					r = f2_fma(f2_mul(c.A0, x0), c.ONE, t);
+				}
+				const u64 u = f2_fma(f2_mul(c.B1, y1), c.ONE, f2_mul(c.B2, y2));
+				y0 = f2_fma(r, c.ONE, u);
+				x2 = x1; x1 = x0; y2 = y1; y1 = y0;
+			}
+		}
+		phi += (uint32_t)OS * dphi;
+		dec[(size_t)g * n_chp] = make_float2(f2_lo(y0), f2_hi(y0));
+	}
+}
+
+template<bool SYM>
+__global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_mixed(vdl2_k1_params p) {
+	constexpr int NLUT = 8;
+	extern __shared__ __align__(128) unsigned char k1m_smem[];
+	const uint32_t TG = p.rx_tile, R = vdl2_rx_tile_stride(TG * p.rx_os_max);
+	const uint32_t rx0 = p.block_rx[2 * blockIdx.x], G = p.block_rx[2 * blockIdx.x + 1];
+	float2 *s_tiles = reinterpret_cast<float2 *>(k1m_smem);                                         /* [2][G][R] */
+	float4 *s_lut = reinterpret_cast<float4 *>(k1m_smem + (size_t)2 * G * R * 8);                   /* [257][8] */
+	uint64_t *s_bar = reinterpret_cast<uint64_t *>(k1m_smem + (size_t)2 * G * R * 8 + 257 * NLUT * 16);
+	const uint32_t tid = threadIdx.x, lane = tid & 31u;
+	const int trace_k = tid == 0 ? vdl2_trace_begin(p.trace_blocks, 1) : -1;
+	const uint32_t ch = blockIdx.x * VDL2_RX_K1_BLOCK + tid;
+	uint32_t chan;
+	const bool active = vdl2_slot_channel(ch, p.lanes, p.full_warps, p.n_ch, chan);
+	const uint32_t row = p.slot_rx[ch] - rx0;                                /* this lane's receiver within the block */
+	const uint32_t cls = p.slot_cls[ch];                                     /* ... and its rate class */
+	const uint32_t n_dec = p.ca ? p.ca->n_pairs : p.n_pairs;                 /* decimated samples per receiver */
+	const size_t stride = p.stream_stride;
+	const float2 *plane = p.samples + (size_t)rx0 * stride;                  /* the block's first receiver */
+	for(uint32_t i = tid; i < 257 * NLUT; i += VDL2_RX_K1_BLOCK) s_lut[i] = p.lut[i / NLUT];
+	const uint32_t lane_bytes = (tid & (NLUT - 1)) * 16u;
+	if(tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
+	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
+	uint32_t phi = 0, dphi = 0;
+	if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
+	u64 x1 = f2_pack(xr1, xi1), x2 = f2_pack(xr2, xi2), y1 = f2_pack(yr1, yi1), y2 = f2_pack(yr2, yi2);
+	auto tap = [&](int j) { return cls == 0 ? p.cls_taps[0][j] : cls == 1 ? p.cls_taps[1][j] : p.cls_taps[2][j]; };
+	const float a0 = tap(0), a1 = tap(1), a2 = tap(2), b1 = tap(3), b2 = tap(4);
+	k1_packed_consts c;
+	c.ONE = f2_pack(p.one, p.one); c.SGN = f2_pack(p.neg_one, p.one);
+	c.A0 = f2_pack(a0, a0); c.A1 = f2_pack(a1, a1); c.A2 = f2_pack(a2, a2);
+	c.B1 = f2_pack(b1, b1); c.B2 = f2_pack(b2, b2); c.TWO = f2_pack(p.two, p.two);
+	c.one = p.one; c.neg_one = p.neg_one;
+	__syncthreads();
+
+	u64 P1 = f2_mul(c.A0, x1), P2 = f2_mul(c.A0, x2);
+	const uint32_t n_tiles = (n_dec + TG - 1) / TG;
+	auto request_tile = [&](uint32_t t, uint32_t buf) {              /* warp 0 */
+		const uint32_t ng = min(TG, n_dec - t * TG);
+		uint32_t mine = 0;
+		for(uint32_t r = lane; r < G; r += 32) mine += ((ng * p.rx_in[rx0 + r].oversample) & ~1u) * (uint32_t)sizeof(float2);
+		const uint32_t bytes = __reduce_add_sync(0xFFFFFFFFu, mine);
+		if(lane == 0) mbar_expect_tx(&s_bar[buf], bytes);
+		__syncwarp();
+		for(uint32_t r = lane; r < G; r += 32) {
+			const uint32_t os_r = p.rx_in[rx0 + r].oversample, n = ng * os_r;
+			const float2 *src = plane + (size_t)r * stride + (size_t)t * TG * os_r;
+			float2 *dst = s_tiles + ((size_t)buf * G + r) * R;
+			tma_copy(dst, src, (n & ~1u) * (uint32_t)sizeof(float2), &s_bar[buf]);
+			if(n & 1u) dst[n - 1] = src[n - 1];
+		}
+	};
+	if(tid < 32)
+		for(uint32_t t = 0; t < 2 && t < n_tiles; t++) request_tile(t, t);
+	__syncthreads();
+	for(uint32_t g0 = 0, tile = 0; g0 < n_dec; g0 += TG, tile++) {
+		const uint32_t ng = min(TG, n_dec - g0);
+		const float2 *s_row = s_tiles + ((size_t)(tile & 1u) * G + row) * R;
+		mbar_wait(&s_bar[tile & 1u], (tile >> 1) & 1u);
+		if(active) {
+			float2 *dec = p.dec + (size_t)g0 * p.n_chp + ch;
+			if(cls == 0) k1m_groups<10, SYM>(s_row, ng, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
+			else if(cls == 1) k1m_groups<13, SYM>(s_row, ng, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
+			else k1m_groups<20, SYM>(s_row, ng, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
+		}
+		__syncthreads();                                           /* every warp is done with this buffer */
+		if(tid < 32 && tile + 2 < n_tiles) request_tile(tile + 2, tile & 1u);
+	}
+	if(active) k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);
+}
+
+/* ------------------------------------------------------------------------------------------------
  * K2: one thread per channel walks the chunk's decimated samples through the demodulator state
  * machine (vdl2_demod_step).  The 160-deep phase ring lives in shared memory, one column per thread
  * (bank = lane, conflict-free whatever the per-channel ring position).
@@ -1328,6 +1486,11 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		cudaFuncSetAttribute(k1_mix_iir_decimate_groups<OS, SYM>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_K1_SMEM_BUDGET); } while(0)
 		K1G_SETUP(20, true); K1G_SETUP(20, false); K1G_SETUP(10, true); K1G_SETUP(10, false); K1G_SETUP(13, true); K1G_SETUP(13, false);
 #undef K1G_SETUP
+		vdl2_set_carveout(k0_convert_mixed, pct);
+		vdl2_set_carveout(k1_mix_iir_decimate_mixed<true>, pct);
+		vdl2_set_carveout(k1_mix_iir_decimate_mixed<false>, pct);
+		cudaFuncSetAttribute(k1_mix_iir_decimate_mixed<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
+		cudaFuncSetAttribute(k1_mix_iir_decimate_mixed<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
 		vdl2_set_carveout(k2a_phase_mag<true>, pct);
 		vdl2_set_carveout(k2a_phase_mag_warps<true>, pct);
 		vdl2_set_carveout(k2a_phase_mag_warps<false>, pct);
@@ -1362,6 +1525,14 @@ extern "C" int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t 
 	return (int)cudaGetLastError();
 }
 
+extern "C" int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *rx, uint32_t n_rx, uint32_t os_max, const float *levels,
+		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st) {
+	if(n_dec == 0 || n_rx == 0) return 0;
+	k0_convert_mixed<<<dim3((n_dec * os_max + 255) / 256, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), n_dec, rx, levels,
+			reinterpret_cast<float2 *>(out2), out_stride, ca);
+	return (int)cudaGetLastError();
+}
+
 template<int OS, int BLOCK>
 static void k1_launch_packed(const vdl2_k1_params *p, int variant, bool sym, cudaStream_t st) {
 	const uint32_t blocks = (p->n_chp + BLOCK - 1) / BLOCK;
@@ -1386,6 +1557,18 @@ extern "C" int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, 
 extern "C" int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st) {
 	if(p->n_pairs == 0 || p->n_ch == 0) return 0;
 	const bool sym = (p->a1 == 2.0f * p->a0) && (p->a2 == p->a0) && variant != 4;
+	if(p->rx_in) {                                    /* mixed-rate receivers: n_pairs counts decimated samples */
+		const uint32_t blocks = (p->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
+		const uint32_t smem = vdl2_rx_k1_smem_bytes(p->rx_max, p->rx_tile * p->rx_os_max);
+		if(p->rx_tile < 2 || p->rx_tile % 2 != 0 || smem > VDL2_RX_MIXED_SMEM_MAX) return (int)cudaErrorInvalidValue;
+		/* the symmetric-tap form only if every rate class present has taps {A0, 2 A0, A0} */
+		bool msym = variant != 4;
+		for(int k = 0; k < 3; k++)
+			if(p->cls_mask & (1u << k)) msym = msym && p->cls_taps[k][1] == 2.0f * p->cls_taps[k][0] && p->cls_taps[k][2] == p->cls_taps[k][0];
+		if(msym) k1_mix_iir_decimate_mixed<true><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p);
+		else k1_mix_iir_decimate_mixed<false><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p);
+		return (int)cudaGetLastError();
+	}
 	if(p->slot_rx) {                                  /* multi-receiver context: samples are float2[n_rx][stream_stride] */
 		const uint32_t blocks = (p->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
 		const uint32_t smem = vdl2_rx_k1_smem_bytes(p->rx_max, p->rx_tile);

@@ -62,6 +62,14 @@ typedef struct {
 	const uint32_t *slot_rx;
 	const uint32_t *block_rx;
 	uint32_t rx_tile, rx_max;
+	/* mixed-rate receivers (vdl2gpu_create_mixed_receivers; NULL otherwise): n_pairs (or ca->n_pairs) counts DECIMATED
+	 * samples per receiver, receiver r has rx_in[r].oversample x n_pairs samples in its row; slot_cls[slot] = rate class
+	 * (vdl2_rx_class) of the slot's receiver, cls_taps[k] = {a0, a1, a2, b1, b2} of class k, cls_mask = the classes present;
+	 * every tile stages rx_tile decimation groups of each receiver, rows of vdl2_rx_tile_stride(rx_tile x rx_os_max) */
+	const vdl2_rx_input *rx_in;
+	const uint8_t *slot_cls;
+	float cls_taps[3][5];
+	uint32_t cls_mask, rx_os_max;
 } vdl2_k1_params;
 
 typedef struct {
@@ -128,6 +136,10 @@ int vdl2_launch_k0(const void *raw, uint32_t n_pairs, uint32_t fmt, const float 
 /* one stream per channel: raw[s][i] -> out2[i][out_stride] float2, time-major across streams */
 int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t fmt, const float *levels, float *out2, uint32_t n_streams,
 		uint32_t raw_stride, uint32_t out_stride, uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *ca, cudaStream_t st);
+/* mixed-rate receivers: row r converts n_dec x rx[r].oversample samples in format rx[r].fmt from raw + n_dec x
+ * rx[r].off_per_dec into out2 + r x out_stride float2 (n_dec from ca->n_pairs when ca is given) */
+int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *rx, uint32_t n_rx, uint32_t os_max, const float *levels,
+		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
 int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st);
 /* whether vdl2_launch_k1 with these arguments runs a kernel that honours p->phase (the pipelined packed kernel with
  * 128-channel blocks); everything else, the receiver-group kernel included, leaves the phase plane to K2a */

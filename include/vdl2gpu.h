@@ -98,7 +98,7 @@ typedef void (*vdl2gpu_frame_cb)(const vdl2gpu_frame *frame, void *user);
 /* per-context counters; names follow the reference's statsd counters (src/statsd.c:33-64) */
 typedef struct {
 	uint64_t chunks_submitted, chunks_completed;
-	uint64_t iq_samples;                 /* complex samples accepted */
+	uint64_t iq_samples;                 /* complex samples accepted (per stream; a mixed-receivers context: of all receivers) */
 	uint64_t dec_samples;                /* decimated samples produced per channel */
 	uint64_t demod_sync_good;            /* demod.sync.good */
 	uint64_t decoder_crc_good;           /* decoder.crc.good (header syndrome 0) */
@@ -141,6 +141,23 @@ typedef struct {
 	uint32_t n_channels;         /* >= 1; this receiver's channels are the next n_channels entries of cfg->freqs */
 } vdl2gpu_receiver;
 int vdl2gpu_create_receivers(const vdl2gpu_config *cfg, const vdl2gpu_receiver *rx, uint32_t n_rx, vdl2gpu_ctx **out);
+/* Receivers of different sample rates and formats in one context (e.g. RTL-SDR dongles, cu8 at 1.05 Msps, next to
+ * SDRplay devices, cs16 at 2.1 Msps): as vdl2gpu_create_receivers, but receiver r samples at 105000 x rx[r].oversample
+ * in format rx[r].sample_fmt, and its filter taps and NCO steps are those of one reference process at that rate.
+ * cfg->sample_rate, oversample, sample_fmt and centerfreq must be 0 (they are per receiver here), cfg->n_streams is 0 or
+ * n_rx, n_rx <= 65535, VDL2GPU_FLAG_K1_SCALAR is refused.  The receivers advance in lock step in DECIMATED samples:
+ * feed the context with vdl2gpu_submit_span / vdl2gpu_submit_span_device (vdl2gpu_submit, vdl2gpu_submit_device and
+ * vdl2gpu_submit_planar_s16 return VDL2GPU_EINVAL).  max_chunk_bytes bounds the buffer of any one receiver in a span:
+ * n_dec <= max_chunk_bytes / max over r of (oversample_r x bytes per complex sample_r).  vdl2gpu_get_tables returns
+ * VDL2GPU_EINVAL (there is no single rate); stats.iq_samples counts the complex samples of all receivers.  Listing the
+ * receivers grouped by rate keeps the 32 channels of a K1 warp on one rate, which runs faster than interleaved rates. */
+typedef struct {
+	uint32_t centerfreq;         /* Hz */
+	uint32_t n_channels;         /* >= 1; the next n_channels entries of cfg->freqs */
+	uint32_t oversample;         /* 10, 13 or 20: this receiver samples at 105000 x oversample */
+	uint32_t sample_fmt;         /* VDL2GPU_FMT_U8 or VDL2GPU_FMT_S16_LE */
+} vdl2gpu_receiver_ex;
+int vdl2gpu_create_mixed_receivers(const vdl2gpu_config *cfg, const vdl2gpu_receiver_ex *rx, uint32_t n_rx, vdl2gpu_ctx **out);
 int vdl2gpu_destroy(vdl2gpu_ctx *ctx);
 const char *vdl2gpu_strerror(int code);
 const char *vdl2gpu_last_error(void);
@@ -160,6 +177,15 @@ int vdl2gpu_submit_planar_s16(vdl2gpu_ctx *ctx, const int16_t *xi, const int16_t
  * was produced; the library orders its work after it.  The buffer may be overwritten once
  * vdl2gpu_wait_input_consumed() has been enqueued on the stream that overwrites it. */
 int vdl2gpu_submit_device(vdl2gpu_ctx *ctx, const void *dev_iq, uint32_t len, void *producer_stream);
+/* One span of n_dec decimated samples for every receiver of a receivers context (vdl2gpu_create_mixed_receivers or
+ * vdl2gpu_create_receivers): receiver r contributes n_dec x oversample_r complex samples in its own format, and the n_rx
+ * buffers lie back to back, receiver 0 first, so receiver r's buffer starts n_dec x sum over q < r of
+ * (oversample_q x bytes per complex sample_q) bytes in (a 64-bit offset).  n_dec == 0 is a no-op; a span longer than
+ * max_chunk_bytes allows returns VDL2GPU_ETOOBIG.  On a vdl2gpu_create_receivers context this is vdl2gpu_submit /
+ * vdl2gpu_submit_device with len = n_dec x oversample x bytes per complex sample; other contexts return VDL2GPU_EINVAL.
+ * Same buffer and stream rules as vdl2gpu_submit / vdl2gpu_submit_device. */
+int vdl2gpu_submit_span(vdl2gpu_ctx *ctx, const void *iq, uint32_t n_dec);
+int vdl2gpu_submit_span_device(vdl2gpu_ctx *ctx, const void *dev_iq, uint32_t n_dec, void *producer_stream);
 int vdl2gpu_wait_input_consumed(vdl2gpu_ctx *ctx, void *stream);
 /* Make `stream` (cudaStream_t) wait for all device work enqueued by this context so far (for timing with
  * events recorded on the caller's stream, and for ordering consumers of device-side results). */
