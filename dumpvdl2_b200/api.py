@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvdl2gpu.so")
 FMT_U8, FMT_S16 = 0, 1
-FLAG_TRACE, FLAG_KEEP_DEC, FLAG_K1_SCALAR, FLAG_NO_OVERLAP, FLAG_NO_GRAPH = 1, 2, 4, 8, 16
+FLAG_TRACE, FLAG_KEEP_DEC, FLAG_K1_SCALAR, FLAG_NO_OVERLAP, FLAG_NO_GRAPH, FLAG_RAGGED = 1, 2, 4, 8, 16, 32
 NUM_COUNTERS = 9
 COUNTER_NAMES = ["sync_good", "hdr_crc_good", "bursts", "burst_err", "blocks_processed",
                  "blocks_fec_ok", "msg_good", "fcs_good", "fcs_bad"]
@@ -82,6 +82,9 @@ def load_library():
     L.vdl2gpu_create_mixed_receivers.argtypes = [C.POINTER(_Config), C.POINTER(_ReceiverEx), C.c_uint32, C.POINTER(C.c_void_p)]
     L.vdl2gpu_submit_span.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_submit_span_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+    L.vdl2gpu_submit_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.vdl2gpu_submit_ragged_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.vdl2gpu_get_receiver_positions.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_destroy.argtypes = [C.c_void_p]
     L.vdl2gpu_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
@@ -403,10 +406,17 @@ class Vdl2MixedReceivers(Vdl2Receivers):
     SDRplay devices, cs16 at 2.1 Msps); every receiver decodes exactly as one reference process at its own rate, tuned to
     its own centre, would.  The receivers advance in lock step in decimated samples (105000 per second for every rate):
     submit_span() takes one buffer per receiver, receiver r's holding n_dec x oversample_r complex samples in its own
-    format.  Listing the receivers grouped by rate keeps every K1 warp on one rate (faster than interleaved rates)."""
+    format.  Listing the receivers grouped by rate keeps every K1 warp on one rate (faster than interleaved rates).
 
-    def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4):
+    With ragged=True the receivers do not advance in lock step: submit_ragged() takes whatever whole decimation groups each
+    receiver has (any count, 0 included, per receiver and per span), and every receiver still decodes exactly what one
+    reference process decodes from the concatenation of its buffers."""
+
+    def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, ragged=False):
         """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16))"""
+        if ragged:
+            flags |= FLAG_RAGGED
+        self.ragged = bool(flags & FLAG_RAGGED)
         self.L = load_library()
         rxs = [(int(cf), [int(f) for f in fr], int(os_), int(fmt)) for cf, fr, os_, fmt in receivers]
         self.receivers = [(cf, fr) for cf, fr, _, _ in rxs]
@@ -466,3 +476,44 @@ class Vdl2MixedReceivers(Vdl2Receivers):
         for d0 in range(0, total, n_dec):
             d1 = min(total, d0 + n_dec)
             self.submit_span([p[d0 * w:d1 * w] for p, w in zip(parts, self.bytes_per_dec)])
+
+    # ---- ragged spans (ragged=True) ----
+    def submit_ragged(self, bufs):
+        """one uint8 buffer per receiver, each a whole number of decimation groups (oversample_r complex samples in the
+        receiver's format; an empty buffer is allowed): receiver r brings len(bufs[r]) / bytes_per_dec[r] decimated samples"""
+        if len(bufs) != self.n_receivers:
+            raise ValueError(f"{len(bufs)} buffers for {self.n_receivers} receivers")
+        parts = [np.ascontiguousarray(b).view(np.uint8).reshape(-1) for b in bufs]
+        for r, p in enumerate(parts):
+            if p.size % self.bytes_per_dec[r]:
+                raise ValueError(f"receiver {r}: {p.size} bytes is not a whole number of decimation groups of {self.bytes_per_dec[r]} bytes")
+        counts = np.array([p.size // w for p, w in zip(parts, self.bytes_per_dec)], np.uint32)
+        buf = np.concatenate(parts) if parts else np.zeros(0, np.uint8)
+        _check(self.L, self.L.vdl2gpu_submit_ragged(self.h, buf.ctypes.data if buf.size else None, counts.ctypes.data), "vdl2gpu_submit_ragged")
+
+    def submit_ragged_device(self, dev_ptr, counts, producer_stream=0):
+        """the receivers' buffers back to back in device memory (receiver 0 first), counts[r] decimated samples of receiver r"""
+        n = np.ascontiguousarray(counts, np.uint32)
+        if n.size != self.n_receivers:
+            raise ValueError(f"{n.size} counts for {self.n_receivers} receivers")
+        _check(self.L, self.L.vdl2gpu_submit_ragged_device(self.h, C.c_void_p(dev_ptr), n.ctypes.data, C.c_void_p(producer_stream)),
+               "vdl2gpu_submit_ragged_device")
+
+    def receiver_positions(self):
+        """decimated samples accepted so far per receiver (uint64[n_receivers])"""
+        out = np.zeros(self.n_receivers, np.uint64)
+        _check(self.L, self.L.vdl2gpu_get_receiver_positions(self.h, out.ctypes.data, self.n_receivers), "vdl2gpu_get_receiver_positions")
+        return out
+
+    def process_ragged(self, bufs, counts_per_span):
+        """each receiver's whole stream, cut into ragged spans: span k brings counts_per_span[k][r] decimated samples of
+        receiver r (a count past the end of that receiver's stream brings what is left)"""
+        parts = [np.ascontiguousarray(b).view(np.uint8).reshape(-1) for b in bufs]
+        pos = [0] * len(parts)
+        for counts in counts_per_span:
+            span = []
+            for r, (p, w) in enumerate(zip(parts, self.bytes_per_dec)):
+                n = min(int(counts[r]), p.size // w - pos[r])
+                span.append(p[pos[r] * w:(pos[r] + n) * w])
+                pos[r] += n
+            self.submit_ragged(span)

@@ -1236,4 +1236,52 @@ VDL2_HD uint32_t vdl2_rx_mixed_tile_groups(uint32_t G, uint32_t os_max) {
 }
 #define VDL2_RX_MIXED_SMEM_MAX (2u * VDL2_RX_K1_BLOCK * (40u + 10u) * 8u + VDL2_RX_K1_LUT_BYTES + 16u)   /* G = 128, TG = 2, os 20 */
 
+/* ------------------------------------------------------------------------------------------------
+ * Ragged spans (VDL2GPU_FLAG_RAGGED on a mixed-receivers context): receiver r brings its own number n_r >= 0 of decimated
+ * samples to every span, and the chain walks each receiver's lanes to that count
+ * ---------------------------------------------------------------------------------------------- */
+/* one receiver's entry of a span's receiver table: where its buffer starts in the span, the decimated samples it brings to
+ * this span (n) and brought to the previous one (prev_n), and its position before this span (dec_base: decimated samples
+ * accepted so far, the index of its first sample in this span) */
+typedef struct {
+	uint64_t off;
+	uint32_t n, prev_n;
+	uint64_t dec_base;
+} vdl2_rx_span;
+
+/* The table of one span from the counts n[r]: the buffers lie back to back, receiver 0 first, n[r] x os_r x bytes per
+ * complex sample each (64-bit offsets).  pos[r] (decimated samples accepted so far) and prev[r] (the count of the previous
+ * span) carry over from span to span: read into the table, then advanced.  Returns the bytes of the span. */
+VDL2_HD uint64_t vdl2_rx_span_table(const vdl2_rx_input *rx, uint32_t n_rx, const uint32_t *n, uint64_t *pos, uint32_t *prev,
+		vdl2_rx_span *out) {
+	uint64_t off = 0;
+	for(uint32_t r = 0; r < n_rx; r++) {
+		out[r].off = off;
+		out[r].n = n[r];
+		out[r].prev_n = prev[r];
+		out[r].dec_base = pos[r];
+		off += (uint64_t)n[r] * rx[r].oversample * (rx[r].fmt == 1u ? 4u : 2u);
+		pos[r] += n[r];
+		prev[r] = n[r];
+	}
+	return off;
+}
+
+/* What row r of the ragged K1's tile at decimation group g0 stages: the groups receiver r still has in the tile,
+ * clamp(n_r - g0, 0, TG), i.e. `samples` = groups x os_r samples; a bulk copy of the even part (`bytes`, 0 = no copy is
+ * issued) and, for an odd count (oversample 13), the last sample copied by hand.  g0 is a multiple of the even TG, so
+ * every copy starts 16-byte aligned, as in the lock-step kernel. */
+typedef struct {
+	uint32_t groups, samples, bytes, odd;
+} vdl2_rx_tile_row;
+
+VDL2_HD vdl2_rx_tile_row vdl2_rx_ragged_row(uint32_t n_r, uint32_t g0, uint32_t TG, uint32_t os_r) {
+	vdl2_rx_tile_row t;
+	t.groups = n_r > g0 ? (n_r - g0 < TG ? n_r - g0 : TG) : 0u;
+	t.samples = t.groups * os_r;
+	t.bytes = (t.samples & ~1u) * 8u;                  /* float2 */
+	t.odd = t.samples & 1u;
+	return t;
+}
+
 #endif

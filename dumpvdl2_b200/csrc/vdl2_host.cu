@@ -57,6 +57,8 @@ struct chunk_slot {
 	/* per-chunk arguments (pinned host copy, device copy made by the first node of the front graph) and the three
 	 * CUDA graphs of this slot per decimated-sample buffer: front {args copy, K0, K1}, K2a, back {K2, history, K3, finish} */
 	vdl2_chunk_args *h_args = nullptr, *d_args = nullptr;
+	/* ragged spans: the span's receiver table (vdl2_rx_span_table; pinned host copy, device copy made with the arguments) */
+	vdl2_rx_span *h_span = nullptr, *d_span = nullptr;
 	cudaGraphExec_t g_front[6] = { nullptr }, g_k2a[6] = { nullptr }, g_back[6] = { nullptr };    /* index = chunk number mod 6 (dec buffer, plane) */
 	uint32_t graph_pairs[6] = { 0 };
 	uint64_t first_pair = 0, dec_base = 0;
@@ -99,6 +101,12 @@ struct vdl2gpu_ctx {
 	uint64_t span_bytes_per_dec = 0, span_pairs_per_dec = 0;   /* sums over the receivers of os x bytes per sample, of os */
 	uint32_t max_span = 0, rx_os_max = 0, cls_mask = 0;  /* largest n_dec of a span; largest oversample; rate classes present */
 	float cls_taps[3][5] = {};                          /* {a0, a1, a2, b1, b2} per rate class (10, 13, 20) */
+	/* ragged spans (VDL2GPU_FLAG_RAGGED on a mixed context): every receiver brings its own count n_r to a span; the chain then
+	 * counts the span's width (the largest n_r) and each kernel lane takes its receiver's entry of the span's table */
+	bool ragged = false;
+	std::vector<uint64_t> rx_pos;                       /* per receiver: decimated samples accepted so far */
+	std::vector<uint32_t> rx_prev;                      /* per receiver: its count in the previous span */
+	std::vector<uint32_t> ch_rx;                        /* per channel: its receiver (burst timestamps) */
 	uint32_t raw_bytes = 0;                             /* size of each slot's raw staging buffers (allocated on the first host submit) */
 	int k1_variant = 2, k2_variant = 5, k2a_mode = 1;   /* A/B knobs (VDL2GPU_K1_VARIANT, VDL2GPU_K2_VARIANT, VDL2GPU_K2A), read at create */
 	bool use_graphs = true;
@@ -195,6 +203,8 @@ static int free_ctx(vdl2gpu_ctx *c) {
 		}
 		if(s.h_args) cudaFreeHost(s.h_args);
 		if(s.d_args) cudaFree(s.d_args);
+		if(s.h_span) cudaFreeHost(s.h_span);
+		if(s.d_span) cudaFree(s.d_span);
 	}
 	cudaFree(c->d_tab); cudaFree(c->d_samples);
 	for(int i = 0; i < 3; i++) cudaFree(c->d_dec3[i]);
@@ -241,6 +251,7 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	c->cfg = *cfg;
 	c->receivers = rx != nullptr;
 	c->mixed = rx_ex != nullptr;
+	c->ragged = c->mixed && (cfg->flags & VDL2GPU_FLAG_RAGGED);
 	c->n_streams = c->receivers ? n_rx : cfg->n_streams ? cfg->n_streams : 1u;
 	c->cfg.n_streams = c->n_streams;
 	c->lane_streams = !c->receivers && c->n_streams > 1 && c->n_streams == cfg->n_channels;     /* one stream per channel */
@@ -424,6 +435,12 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 			CU(cudaMemcpy(c->d_rx_in, c->rx_in.data(), c->rx_in.size() * sizeof(vdl2_rx_input), cudaMemcpyHostToDevice));
 			CU(cudaMemcpy(c->d_slot_cls, slot_cls.data(), slot_cls.size(), cudaMemcpyHostToDevice));
 		}
+		if(c->ragged) {
+			c->rx_pos.assign(n_rx, 0);
+			c->rx_prev.assign(n_rx, 0);
+			c->ch_rx.resize(c->n_ch);
+			for(uint32_t r = 0; r < n_rx; r++) std::fill(c->ch_rx.begin() + rx_first[r], c->ch_rx.begin() + rx_first[r + 1], r);
+		}
 	}
 	initial_state(c->cfg, c->freqs.data(), c->receivers ? centres.data() : nullptr, c->mixed ? rates.data() : nullptr, c->n_ch, c->n_chp,
 			c->lanes, c->full_warps, k1, k2);
@@ -443,6 +460,10 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 		 * use vdl2gpu_submit_device never need them */
 		CU(cudaHostAlloc((void **)&s.h_args, sizeof(vdl2_chunk_args), cudaHostAllocDefault));
 		CU(cudaMalloc(&s.d_args, sizeof(vdl2_chunk_args)));
+		if(c->ragged) {
+			CU(cudaHostAlloc((void **)&s.h_span, (size_t)n_rx * sizeof(vdl2_rx_span), cudaHostAllocDefault));
+			CU(cudaMalloc(&s.d_span, (size_t)n_rx * sizeof(vdl2_rx_span)));
+		}
 		CU(cudaHostAlloc((void **)&s.h_out, sizeof(vdl2_out_header) + c->out_cap, cudaHostAllocMapped));
 		CU(cudaHostGetDevicePointer((void **)&s.d_out, s.h_out, 0));
 		memset(s.h_out, 0, sizeof(vdl2_out_header));
@@ -452,12 +473,21 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	return VDL2GPU_OK;
 }
 
+/* VDL2GPU_FLAG_RAGGED outside vdl2gpu_create_mixed_receivers: refused rather than ignored, since ignoring it would give the
+ * caller lock-step spans they did not ask for */
+static int refuse_ragged(const char *what) {
+	snprintf(g_last_error, sizeof(g_last_error), "%s: VDL2GPU_FLAG_RAGGED needs vdl2gpu_create_mixed_receivers "
+			"(a uniform fleet gets ragged spans by describing itself there)", what);
+	return VDL2GPU_EINVAL;
+}
+
 extern "C" int vdl2gpu_create(const vdl2gpu_config *cfg, vdl2gpu_ctx **out) {
 	if(!cfg || !out || !cfg->freqs || cfg->n_channels == 0 || cfg->oversample == 0 || cfg->sample_fmt > 1
 			|| cfg->sample_rate != (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * cfg->oversample) {
 		snprintf(g_last_error, sizeof(g_last_error), "bad vdl2gpu_config (sample_rate must be 105000*oversample)");
 		return VDL2GPU_EINVAL;
 	}
+	if(cfg->flags & VDL2GPU_FLAG_RAGGED) return refuse_ragged("vdl2gpu_create");
 	vdl2gpu_ctx *c = new vdl2gpu_ctx();
 	int rc = create_impl(cfg, c);
 	if(rc != VDL2GPU_OK) { free_ctx(c); *out = nullptr; return rc; }
@@ -475,7 +505,10 @@ extern "C" int vdl2gpu_create_receivers(const vdl2gpu_config *cfg, const vdl2gpu
 	else if(cfg->n_streams != 0 && cfg->n_streams != n_rx) why = "n_streams must be 0 or the number of receivers";
 	else if(cfg->oversample != 20 && cfg->oversample != 10 && cfg->oversample != 13) why = "receivers need oversample 20, 10 or 13 (the rates the receiver-group K1 is built for)";
 	else if(cfg->flags & VDL2GPU_FLAG_K1_SCALAR) why = "VDL2GPU_FLAG_K1_SCALAR is not available with receivers";
-	else {
+	else if(cfg->flags & VDL2GPU_FLAG_RAGGED) {
+		if(out) *out = nullptr;
+		return refuse_ragged("vdl2gpu_create_receivers");
+	} else {
 		for(uint32_t r = 0; r < n_rx && !why; r++) {
 			if(rx[r].n_channels == 0) why = "a receiver has no channels";
 			sum += rx[r].n_channels;
@@ -542,9 +575,11 @@ static uint32_t synd_weight_of(uint32_t syn) {       /* src/decode.c:98-100 */
 }
 
 /* burst records (region = vdl2_out_header + records) -> frames.  Offsets in the pending frames are relative to the
- * first record.  `dec_end` / `arrival` place the burst in time (see burst_timestamp below). */
+ * first record.  `dec_end` / `arrival` place the burst in time (see burst_timestamp below); with ragged spans `span` (the
+ * span's receiver table) and `ch_rx` (channel -> receiver) give each channel its own receiver's end position instead. */
 static void parse_region(const uint8_t *region, uint32_t out_cap, double rate, struct timeval arrival, uint64_t dec_end,
-		uint32_t blob_id, std::vector<pending_frame> &pending, vdl2gpu_stats &stats) {
+		uint32_t blob_id, std::vector<pending_frame> &pending, vdl2gpu_stats &stats, const vdl2_rx_span *span = nullptr,
+		const uint32_t *ch_rx = nullptr) {
 	vdl2_out_header h;
 	memcpy(&h, region, sizeof(h));
 	const uint8_t *base = region + sizeof(vdl2_out_header);
@@ -573,6 +608,8 @@ static void parse_region(const uint8_t *region, uint32_t out_cap, double rate, s
 		const uint8_t *bytes = reinterpret_cast<const uint8_t *>(tab + r->n_frames);
 		uint32_t foff = 0;
 		const uint64_t sync_idx = (uint64_t)r->sync_lo | ((uint64_t)r->sync_hi << 32);
+		uint64_t end = dec_end;
+		if(span) { const vdl2_rx_span &e = span[ch_rx[r->channel]]; end = e.dec_base + e.n; }
 		for(uint32_t k = 0; k < r->n_frames; k++) {
 			const uint32_t len = tab[k] & 0xFFFFu, crc = tab[k] >> 16;
 			pending_frame pf;
@@ -592,7 +629,7 @@ static void parse_region(const uint8_t *region, uint32_t out_cap, double rate, s
 			pf.f.sync_dec_index = sync_idx;
 			/* the reference stamps gettimeofday() at sync (src/demod.c:246); here: arrival time of the chunk
 			 * being processed when the burst completed, moved back by the distance to the sync sample */
-			double back = dec_end > sync_idx ? ((double)dec_end - (double)sync_idx) / rate : 0.0;
+			double back = end > sync_idx ? ((double)end - (double)sync_idx) / rate : 0.0;
 			double ts = (double)arrival.tv_sec + 1e-6 * (double)arrival.tv_usec - back;
 			pf.f.burst_timestamp.tv_sec = (time_t)floor(ts);
 			pf.f.burst_timestamp.tv_usec = (suseconds_t)((ts - floor(ts)) * 1e6);
@@ -630,7 +667,8 @@ static void harvest(vdl2gpu_ctx *c, chunk_slot &s) {
 	const uint32_t blob_id = (uint32_t)c->blobs.size() - 1;
 	/* decimated samples per second (105000 for every receiver of a mixed context, whose config carries no rate) */
 	const double rate = c->mixed ? (double)VDL2_SYMBOL_RATE * VDL2_SPS : (double)c->cfg.sample_rate / (double)c->cfg.oversample;
-	parse_region(c->blobs.back().data(), c->out_cap, rate, s.arrival, s.dec_base + s.n_dec, blob_id, c->pending, c->stats);
+	parse_region(c->blobs.back().data(), c->out_cap, rate, s.arrival, s.dec_base + s.n_dec, blob_id, c->pending, c->stats,
+			c->ragged ? s.h_span : nullptr, c->ch_rx.data());
 	c->stats.chunks_completed++;
 	s.busy = false;
 }
@@ -713,6 +751,7 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	p2.pool = c->d_pool; p2.free_list = c->d_free; p2.ready = c->d_ready; p2.ctl = c->d_ctl;
 	p2.events = c->d_events; p2.event_cap = c->event_cap; p2.trace = (c->cfg.flags & VDL2GPU_FLAG_TRACE) ? 1u : 0u;
 	p2.variant = (uint32_t)c->k2_variant; p2.k2a_mode = (uint32_t)c->k2a_mode; p2.ca = ca;
+	p1.rx_span = s.d_span; pa.slot_rx = c->d_slot_rx; pa.rx_span = s.d_span; p2.slot_rx = c->d_slot_rx; p2.rx_span = s.d_span;   /* (NULL unless ragged) */
 	p3.pool = c->d_pool; p3.free_list = c->d_free; p3.ready = c->d_ready; p3.ctl = c->d_ctl; p3.tables = c->d_tab;
 	p3.out = s.d_out; p3.out_cap = c->out_cap; p3.n_chp = c->n_chp; p3.counters = c->d_counters;
 }
@@ -745,6 +784,14 @@ static int launch_k0_mixed(vdl2gpu_ctx *c, const void *d_raw, uint32_t n_dec, co
 	return VDL2GPU_OK;
 }
 
+/* mixed-rate receivers: K0 of a span of n_dec decimated samples (ragged spans: n_dec is the width, the slot's table the counts) */
+static int launch_k0_span(vdl2gpu_ctx *c, const chunk_slot &s, const void *d_raw, uint32_t n_dec, const vdl2_chunk_args *ca) {
+	if(!c->ragged) return launch_k0_mixed(c, d_raw, n_dec, ca);
+	KL(vdl2_launch_k0_ragged(d_raw, n_dec, c->d_rx_in, s.d_span, c->n_streams, c->rx_os_max, c->d_tab->levels,
+			reinterpret_cast<float *>(c->d_samples), c->max_pairs, ca, c->stream));
+	return VDL2GPU_OK;
+}
+
 struct capture_env { vdl2gpu_ctx *c; chunk_slot *s; uint64_t seq; uint32_t n_pairs; uint32_t k0_fmt; };
 #define CAPTURE_PARAMS \
 	capture_env *e = static_cast<capture_env *>(a); \
@@ -757,8 +804,9 @@ static int body_front(void *a) {
 	CAPTURE_PARAMS;
 	(void)pa; (void)p2; (void)p3;
 	CU(cudaMemcpyAsync(e->s->d_args, e->s->h_args, sizeof(vdl2_chunk_args), cudaMemcpyHostToDevice, c->stream));
+	if(c->ragged) CU(cudaMemcpyAsync(e->s->d_span, e->s->h_span, c->n_streams * sizeof(vdl2_rx_span), cudaMemcpyHostToDevice, c->stream));
 	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
-	if(c->mixed) { int rc = launch_k0_mixed(c, nullptr, e->n_pairs, e->s->d_args); if(rc) return rc; }
+	if(c->mixed) { int rc = launch_k0_span(c, *e->s, nullptr, e->n_pairs, e->s->d_args); if(rc) return rc; }
 	else if(c->lane_streams) KL(vdl2_launch_k0_lanes(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 			e->n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, e->s->d_args, c->stream));
 	else KL(vdl2_launch_k0(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
@@ -835,7 +883,8 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	if(graph) {
 		CU(cudaGraphLaunch(s.g_front[gk], c->stream));
 	} else {
-		if(c->mixed) { int rc = launch_k0_mixed(c, d_raw, n_pairs, nullptr); if(rc) return rc; }
+		if(c->ragged) CU(cudaMemcpyAsync(s.d_span, s.h_span, c->n_streams * sizeof(vdl2_rx_span), cudaMemcpyHostToDevice, c->stream));
+		if(c->mixed) { int rc = launch_k0_span(c, s, d_raw, n_pairs, nullptr); if(rc) return rc; }
 		else if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 				n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, nullptr, c->stream));
 		else KL(vdl2_launch_k0(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
@@ -883,7 +932,8 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	c->total_dec += s.n_dec;
 	c->last_n_dec = s.n_dec;
 	c->stats.chunks_submitted++;
-	c->stats.iq_samples += c->mixed ? (uint64_t)n_pairs * c->span_pairs_per_dec : n_pairs;
+	if(c->ragged) for(uint32_t r = 0; r < c->n_streams; r++) c->stats.iq_samples += (uint64_t)s.h_span[r].n * c->rx_in[r].oversample;
+	else c->stats.iq_samples += c->mixed ? (uint64_t)n_pairs * c->span_pairs_per_dec : n_pairs;
 	c->stats.dec_samples += s.n_dec;
 	c->stats.kernel_launches += (n_pairs ? 2 : 0) + (c->fuse_phase ? 0 : 1) + (s.n_dec ? 1 : 0) + 2;
 	return VDL2GPU_OK;
@@ -1017,12 +1067,71 @@ static int span_check(vdl2gpu_ctx *c, const void *iq, uint32_t n_dec, const char
 	return 0;
 }
 
+/* Ragged spans: receiver r brings n_dec[r] decimated samples (host buffer, or device buffer ordered after producer_stream).
+ * Everything is checked before the device is touched; the span then runs the chain at its width, the largest count, with
+ * the span's receiver table (built in the slot's pinned copy: the slot's previous chunk has been harvested) telling every
+ * kernel lane its receiver's count, place in the buffer and position. */
+static int ragged_submit(vdl2gpu_ctx *c, const void *iq, const uint32_t *n_dec, bool device, void *producer_stream, const char *what) {
+	if(!c || !n_dec) return VDL2GPU_EINVAL;
+	if(!c->ragged) {
+		snprintf(g_last_error, sizeof(g_last_error), "%s: needs a context made by vdl2gpu_create_mixed_receivers with VDL2GPU_FLAG_RAGGED", what);
+		return VDL2GPU_EINVAL;
+	}
+	uint32_t width = 0;
+	for(uint32_t r = 0; r < c->n_streams; r++) {
+		if(n_dec[r] > c->max_span) {
+			snprintf(g_last_error, sizeof(g_last_error), "%s: receiver %u brings %u decimated samples, at most %u fit max_chunk_bytes", what, r, n_dec[r], c->max_span);
+			return VDL2GPU_ETOOBIG;
+		}
+		width = std::max(width, n_dec[r]);
+	}
+	if(width == 0) return VDL2GPU_OK;
+	if(!iq) return VDL2GPU_EINVAL;
+	CU(cudaSetDevice(c->device));
+	chunk_slot *s;
+	int rc = acquire_slot(c, &s);
+	if(rc) return rc;
+	if(!device) {
+		rc = ensure_raw(c, *s);
+		if(rc) return rc;
+	}
+	/* every buffer is at most max_span x its receiver's bytes per decimated sample <= max_chunk_bytes: the span fits the
+	 * max_chunk_bytes x n_rx staging buffer */
+	const uint64_t bytes = vdl2_rx_span_table(c->rx_in.data(), c->n_streams, n_dec, c->rx_pos.data(), c->rx_prev.data(), s->h_span);
+	if(device) {
+		CU(cudaEventRecord(c->ev_input_ready, (cudaStream_t)producer_stream));
+		CU(cudaStreamWaitEvent(c->stream, c->ev_input_ready, 0));
+		return run_chain(c, *s, iq, width);
+	}
+	memcpy(s->h_raw, iq, bytes);
+	CU(cudaMemcpyAsync(s->d_raw, s->h_raw, bytes, cudaMemcpyHostToDevice, c->stream));
+	return run_chain(c, *s, s->d_raw, width);
+}
+
+extern "C" int vdl2gpu_submit_ragged(vdl2gpu_ctx *c, const void *iq, const uint32_t *n_dec) {
+	return ragged_submit(c, iq, n_dec, false, nullptr, "vdl2gpu_submit_ragged");
+}
+
+extern "C" int vdl2gpu_submit_ragged_device(vdl2gpu_ctx *c, const void *dev_iq, const uint32_t *n_dec, void *producer_stream) {
+	return ragged_submit(c, dev_iq, n_dec, true, producer_stream, "vdl2gpu_submit_ragged_device");
+}
+
+extern "C" int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *c, uint64_t *out, uint32_t n_rx) {
+	if(!c || !out || !c->receivers || n_rx > c->n_streams) return VDL2GPU_EINVAL;
+	for(uint32_t r = 0; r < n_rx; r++) out[r] = c->ragged ? c->rx_pos[r] : c->total_dec;
+	return VDL2GPU_OK;
+}
+
 extern "C" int vdl2gpu_submit_span(vdl2gpu_ctx *c, const void *iq, uint32_t n_dec) {
 	uint32_t len = 0;
 	int rc = span_check(c, iq, n_dec, "vdl2gpu_submit_span", &len);
 	if(rc < 0) return rc;
 	if(rc == 0) return vdl2gpu_submit(c, iq, len);
 	if(n_dec == 0) return VDL2GPU_OK;
+	if(c->ragged) {
+		const std::vector<uint32_t> n(c->n_streams, n_dec);
+		return ragged_submit(c, iq, n.data(), false, nullptr, "vdl2gpu_submit_span");
+	}
 	CU(cudaSetDevice(c->device));
 	chunk_slot *s;
 	rc = acquire_slot(c, &s);
@@ -1042,6 +1151,10 @@ extern "C" int vdl2gpu_submit_span_device(vdl2gpu_ctx *c, const void *dev_iq, ui
 	if(rc < 0) return rc;
 	if(rc == 0) return vdl2gpu_submit_device(c, dev_iq, len, producer_stream);
 	if(n_dec == 0) return VDL2GPU_OK;
+	if(c->ragged) {
+		const std::vector<uint32_t> n(c->n_streams, n_dec);
+		return ragged_submit(c, dev_iq, n.data(), true, producer_stream, "vdl2gpu_submit_span_device");
+	}
 	CU(cudaSetDevice(c->device));
 	chunk_slot *s;
 	rc = acquire_slot(c, &s);
@@ -1404,6 +1517,7 @@ static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, cons
 extern "C" int vdl2gpu_stage_create(const vdl2gpu_config *cfg, uint32_t max_dec, void *device_mem, size_t device_bytes, vdl2gpu_stage **out) {
 	if(!cfg || !out || !device_mem || !cfg->freqs || cfg->n_channels == 0 || cfg->oversample == 0 || max_dec == 0
 			|| cfg->sample_rate != (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * cfg->oversample) return VDL2GPU_EINVAL;
+	if(cfg->flags & VDL2GPU_FLAG_RAGGED) return refuse_ragged("vdl2gpu_stage_create");
 	const uint32_t ecap = stage_event_cap(cfg->flags);
 	const stage_layout L = stage_layout_of(cfg->n_channels, max_dec, ecap);
 	if(device_bytes < L.total || ((uintptr_t)device_mem & 255u)) return VDL2GPU_EINVAL;

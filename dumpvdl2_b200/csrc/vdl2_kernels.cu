@@ -98,13 +98,8 @@ __global__ void __launch_bounds__(1024) k0_convert_lanes(const uint8_t *__restri
 /* K0 for mixed-rate receivers: grid row r converts receiver r's n_dec x os_r samples, in its own format, from its own
  * place in the span (vdl2_rx_span_offset) into row r of the sample plane; the same arithmetic as k0_convert.  Rows of
  * receivers with a smaller oversample factor than the largest leave their surplus threads idle. */
-__global__ void __launch_bounds__(256) k0_convert_mixed(const uint8_t *__restrict__ raw0, uint32_t n_dec_p, const vdl2_rx_input *__restrict__ rx,
-		const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride, const vdl2_chunk_args *__restrict__ ca) {
-	const uint32_t n_dec = ca ? ca->n_pairs : n_dec_p;
-	const vdl2_rx_input in = rx[blockIdx.y];
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if(i >= n_dec * in.oversample) return;
-	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec);
+__device__ __forceinline__ float2 k0_mixed_sample(const uint8_t *__restrict__ raw, const vdl2_rx_input &in, uint32_t i,
+		const float *__restrict__ levels) {
 	float re, im;
 	if(in.fmt == 0) {                                    /* src/demod.c:343-345, table from :349-354 */
 		uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
@@ -118,7 +113,29 @@ __global__ void __launch_bounds__(256) k0_convert_mixed(const uint8_t *__restric
 		re = __fdiv_rn((float)v.x, 32768.0f);
 		im = __fdiv_rn((float)v.y, 32768.0f);
 	}
-	out0[(size_t)blockIdx.y * out_stride + i] = make_float2(re, im);
+	return make_float2(re, im);
+}
+
+__global__ void __launch_bounds__(256) k0_convert_mixed(const uint8_t *__restrict__ raw0, uint32_t n_dec_p, const vdl2_rx_input *__restrict__ rx,
+		const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride, const vdl2_chunk_args *__restrict__ ca) {
+	const uint32_t n_dec = ca ? ca->n_pairs : n_dec_p;
+	const vdl2_rx_input in = rx[blockIdx.y];
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= n_dec * in.oversample) return;
+	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec);
+	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(raw, in, i, levels);
+}
+
+/* K0 on ragged spans: grid row r converts the span[r].n x os_r samples receiver r brought to this span, from its own place
+ * in the span (its entry of the span's receiver table), into row r of the sample plane; rows past their count idle */
+__global__ void __launch_bounds__(256) k0_convert_ragged(const uint8_t *__restrict__ raw0, const vdl2_rx_input *__restrict__ rx,
+		const vdl2_rx_span *__restrict__ span, const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride,
+		const vdl2_chunk_args *__restrict__ ca) {
+	const vdl2_rx_input in = rx[blockIdx.y];
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= span[blockIdx.y].n * in.oversample) return;
+	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + span[blockIdx.y].off;
+	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(raw, in, i, levels);
 }
 
 /* ------------------------------------------------------------------------------------------------
@@ -835,8 +852,20 @@ __device__ __forceinline__ void k1m_groups(const float2 *s_row, uint32_t ng, flo
 	}
 }
 
-template<bool SYM>
-__global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_mixed(vdl2_k1_params p) {
+/* the ragged K1's tile loop bound: the most groups any of the block's G receivers brings to the span (a whole warp calls) */
+__device__ __forceinline__ uint32_t k1r_block_width(const vdl2_rx_span *span, uint32_t G, uint32_t lane) {
+	uint32_t w = 0;
+	for(uint32_t r = lane; r < G; r += 32) w = max(w, span[r].n);
+	return __reduce_max_sync(0xFFFFFFFFu, w);
+}
+
+/* Ragged spans (RAGGED, k1_mix_iir_decimate_ragged): receiver r brings p.rx_span[r].n groups.  The tile loop stays uniform
+ * across the block and runs to the largest count of the block's receivers, which each warp reduces for itself at the
+ * start (no shared slot, no extra barrier).  Row r of the tile at group g0 stages vdl2_rx_ragged_row(n_r, g0, ...): a row
+ * with nothing left issues no copy, and the tile's expected transaction bytes are the sum of the copies issued.  A lane
+ * runs the groups its receiver has in the tile; a lane whose receiver brought nothing neither loads nor stores its state. */
+template<bool SYM, bool RAGGED>
+__device__ __forceinline__ void k1_mixed_body(const vdl2_k1_params &p) {
 	constexpr int NLUT = 8;
 	extern __shared__ __align__(128) unsigned char k1m_smem[];
 	const uint32_t TG = p.rx_tile, R = vdl2_rx_tile_stride(TG * p.rx_os_max);
@@ -848,10 +877,12 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_mixed(vd
 	const int trace_k = tid == 0 ? vdl2_trace_begin(p.trace_blocks, 1) : -1;
 	const uint32_t ch = blockIdx.x * VDL2_RX_K1_BLOCK + tid;
 	uint32_t chan;
-	const bool active = vdl2_slot_channel(ch, p.lanes, p.full_warps, p.n_ch, chan);
+	const bool active = vdl2_slot_channel(ch, p.lanes, p.full_warps, p.n_ch, chan) && (!RAGGED || p.rx_span[p.slot_rx[ch]].n > 0);
 	const uint32_t row = p.slot_rx[ch] - rx0;                                /* this lane's receiver within the block */
 	const uint32_t cls = p.slot_cls[ch];                                     /* ... and its rate class */
-	const uint32_t n_dec = p.ca ? p.ca->n_pairs : p.n_pairs;                 /* decimated samples per receiver */
+	/* decimated samples per receiver (ragged: the most any receiver of the block brings) */
+	const uint32_t n_dec = RAGGED ? k1r_block_width(p.rx_span + rx0, G, lane) : p.ca ? p.ca->n_pairs : p.n_pairs;
+	const uint32_t n_mine = RAGGED ? p.rx_span[rx0 + row].n : n_dec;       /* ... and this lane's receiver brings */
 	const size_t stride = p.stream_stride;
 	const float2 *plane = p.samples + (size_t)rx0 * stride;                  /* the block's first receiver */
 	for(uint32_t i = tid; i < 257 * NLUT; i += VDL2_RX_K1_BLOCK) s_lut[i] = p.lut[i / NLUT];
@@ -875,15 +906,18 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_mixed(vd
 	auto request_tile = [&](uint32_t t, uint32_t buf) {              /* warp 0 */
 		const uint32_t ng = min(TG, n_dec - t * TG);
 		uint32_t mine = 0;
-		for(uint32_t r = lane; r < G; r += 32) mine += ((ng * p.rx_in[rx0 + r].oversample) & ~1u) * (uint32_t)sizeof(float2);
+		for(uint32_t r = lane; r < G; r += 32)
+			mine += RAGGED ? vdl2_rx_ragged_row(p.rx_span[rx0 + r].n, t * TG, TG, p.rx_in[rx0 + r].oversample).bytes
+			               : ((ng * p.rx_in[rx0 + r].oversample) & ~1u) * (uint32_t)sizeof(float2);
 		const uint32_t bytes = __reduce_add_sync(0xFFFFFFFFu, mine);
 		if(lane == 0) mbar_expect_tx(&s_bar[buf], bytes);
 		__syncwarp();
 		for(uint32_t r = lane; r < G; r += 32) {
-			const uint32_t os_r = p.rx_in[rx0 + r].oversample, n = ng * os_r;
+			const uint32_t os_r = p.rx_in[rx0 + r].oversample;
+			const uint32_t n = RAGGED ? vdl2_rx_ragged_row(p.rx_span[rx0 + r].n, t * TG, TG, os_r).samples : ng * os_r;
 			const float2 *src = plane + (size_t)r * stride + (size_t)t * TG * os_r;
 			float2 *dst = s_tiles + ((size_t)buf * G + r) * R;
-			tma_copy(dst, src, (n & ~1u) * (uint32_t)sizeof(float2), &s_bar[buf]);
+			if(!RAGGED || n != 0) tma_copy(dst, src, (n & ~1u) * (uint32_t)sizeof(float2), &s_bar[buf]);
 			if(n & 1u) dst[n - 1] = src[n - 1];
 		}
 	};
@@ -896,9 +930,10 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_mixed(vd
 		mbar_wait(&s_bar[tile & 1u], (tile >> 1) & 1u);
 		if(active) {
 			float2 *dec = p.dec + (size_t)g0 * p.n_chp + ch;
-			if(cls == 0) k1m_groups<10, SYM>(s_row, ng, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
-			else if(cls == 1) k1m_groups<13, SYM>(s_row, ng, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
-			else k1m_groups<20, SYM>(s_row, ng, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
+			const uint32_t nl = RAGGED ? vdl2_rx_ragged_row(n_mine, g0, TG, 1u).groups : ng;      /* (ng: n_mine <= n_dec) */
+			if(cls == 0) k1m_groups<10, SYM>(s_row, nl, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
+			else if(cls == 1) k1m_groups<13, SYM>(s_row, nl, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
+			else k1m_groups<20, SYM>(s_row, nl, dec, p.n_chp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
 		}
 		__syncthreads();                                           /* every warp is done with this buffer */
 		if(tid < 32 && tile + 2 < n_tiles) request_tile(tile + 2, tile & 1u);
@@ -906,6 +941,11 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_mixed(vd
 	if(active) k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
 	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);
 }
+
+template<bool SYM>
+__global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_mixed(vdl2_k1_params p) { k1_mixed_body<SYM, false>(p); }
+template<bool SYM>
+__global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_ragged(vdl2_k1_params p) { k1_mixed_body<SYM, true>(p); }
 
 /* ------------------------------------------------------------------------------------------------
  * K2: one thread per channel walks the chunk's decimated samples through the demodulator state
@@ -958,8 +998,14 @@ __global__ void __launch_bounds__(256) k2a_phase_mag(const float2 *__restrict__ 
  * four at a time (four independent evaluations in flight).  Before that it copies the previous plane's last 160 phase rows
  * into this plane's history rows (the planes alternate between chunks; with n_dec < 160 the source range still lies inside
  * the previous plane, history rows included, so short chunks need no special case). */
-template<bool FAST>
-__global__ void __launch_bounds__(128, 8) k2a_phase_mag_warps(vdl2_k2a_params p) {      /* <= 64 registers: 32 warps per SM */
+/* Ragged spans (RAGGED, k2a_phase_mag_warps_ragged): a lane evaluates the rows its receiver brought, rx_span[r].n, and takes
+ * its history from the previous plane's rows [prev_n, prev_n + 160), prev_n = its receiver's count in the previous span.
+ * That is the last 160 phases of the receiver's stream whatever prev_n is: the previous plane holds, per slot, the 160
+ * history rows it was given followed by that slot's prev_n new rows.  With prev_n = 0 (the receiver brought nothing last
+ * span) the range is the previous plane's own history rows, which are the right ones; with 0 < prev_n < 160 it straddles
+ * history and new rows, still in order.  So the two alternating planes need no change for ragged spans. */
+template<bool FAST, bool RAGGED>
+__device__ __forceinline__ void k2a_warps_body(const vdl2_k2a_params &p) {
 	__shared__ double s_atan[VDL2_ATAN_TABLE_DOUBLES];
 	if(FAST) {
 		if(threadIdx.x < VDL2_ATAN_TABLE_DOUBLES) s_atan[threadIdx.x] = c_atan_tab[threadIdx.x];
@@ -969,10 +1015,12 @@ __global__ void __launch_bounds__(128, 8) k2a_phase_mag_warps(vdl2_k2a_params p)
 	const uint32_t slot = (blockIdx.x % nblk) * 128u + threadIdx.x;
 	uint32_t chan;
 	if(!vdl2_slot_channel(slot, p.lanes, p.full_warps, p.n_ch, chan)) return;
-	const uint32_t n_all = p.ca ? p.ca->n_dec : p.n_dec, prev_n_dec = p.ca ? p.ca->prev_n_dec : p.prev_n_dec;
-	/* this block's time slice [t, n_dec) of the chunk, boundaries on multiples of 4 samples */
+	const uint32_t n_all = p.ca ? p.ca->n_dec : p.n_dec, prev_n_dec = RAGGED ? p.rx_span[p.slot_rx[slot]].prev_n : p.ca ? p.ca->prev_n_dec : p.prev_n_dec;
+	const uint32_t n_mine = RAGGED ? p.rx_span[p.slot_rx[slot]].n : n_all;     /* ragged: n_all is the span's width */
+	/* this block's time slice [t, n_dec) of the chunk, boundaries on multiples of 4 samples (ragged: the width's slices,
+	 * cut at this lane's count: the slice arithmetic stays uniform across the block) */
 	const uint32_t per = ((n_all + p.split - 1u) / p.split + 3u) & ~3u;
-	const uint32_t n_dec = min(n_all, (slice + 1u) * per);
+	const uint32_t n_dec = min(n_mine, (slice + 1u) * per);
 	const size_t s = p.n_chp;
 	if(slice == 0) {
 		const float *src = p.phase_prev + (size_t)prev_n_dec * s + slot;
@@ -982,7 +1030,7 @@ __global__ void __launch_bounds__(128, 8) k2a_phase_mag_warps(vdl2_k2a_params p)
 	}
 	const float2 *dec = p.dec + slot;
 	float *ph = p.phase + (size_t)VDL2_SYNC_BUFLEN * s + slot, *mg = p.mag + slot;
-	uint32_t t = min(n_all, slice * per);
+	uint32_t t = min(n_mine, slice * per);
 	const bool want_mag = p.mag != nullptr;
 	/* four samples per step; the next four are requested before the current four are evaluated, so that the loads'
 	 * latency hides behind ~400 instructions of arithmetic (the kernel was long-scoreboard bound without it).  FAST: the
@@ -1025,6 +1073,13 @@ __global__ void __launch_bounds__(128, 8) k2a_phase_mag_warps(vdl2_k2a_params p)
 	}
 }
 
+template<bool FAST>
+__global__ void __launch_bounds__(128, 8) k2a_phase_mag_warps(vdl2_k2a_params p) { k2a_warps_body<FAST, false>(p); }     /* <= 64 registers: 32 warps per SM */
+/* (the lane's own row count and slice end take two more registers than the uniform ones of the lock-step kernel: within 64
+ * the fast form spilled, so seven blocks per SM, <= 72 registers) */
+template<bool FAST>
+__global__ void __launch_bounds__(128, 7) k2a_phase_mag_warps_ragged(vdl2_k2a_params p) { k2a_warps_body<FAST, true>(p); }
+
 /* carry the last 160 phase rows over to the front of the plane for the next chunk: rows [n_dec, n_dec+160) -> [0, 160) */
 __global__ void __launch_bounds__(256) k_copy_rows(const float *__restrict__ src, float *__restrict__ dst, uint32_t n) {
 	uint32_t i = blockIdx.x * 256u + threadIdx.x;
@@ -1059,8 +1114,13 @@ __device__ __forceinline__ void k2_cp_async_wait_all() { asm volatile("cp.async.
 #define K2_STAGE_FLOATS(MODE) ((MODE) == 4 ? 2 * (VDL2_WALK_BLOCK + 2 * VDL2_WALK_BLOCK) : (MODE) == 3 ? 2 * 16 : 0)
 #define K2_SMEM_BYTES(BLOCK, MODE) ((VDL2_SYNC_BUFLEN + K2_STAGE_FLOATS(MODE)) * (BLOCK) * 4 + 36 * 4 + VDL2_UNWRAP_STATES * 6 * 4)
 
-template<int BLOCK, bool BLOCKED, int MODE>
-__global__ void __launch_bounds__(BLOCK) k2_sync_slice(vdl2_k2_params p) {
+/* RAGGED (k2_sync_slice_ragged): the lane walks the samples its receiver brought to the span, rx_span[r].n, and numbers them
+ * from rx_span[r].dec_base, i.e. in the receiver's own decimated samples.  Legal because after the barrier that loads the
+ * constants there is no block-wide barrier left, the cp.async staging copies each thread's own column, and the walk
+ * functions of vdl2_core.cuh use no warp-synchronous intrinsics: each lane's loop bound is its own.  A lane whose receiver
+ * brought nothing loads and stores its state unchanged. */
+template<int BLOCK, bool BLOCKED, int MODE, bool RAGGED>
+__device__ __forceinline__ void k2_sync_body(const vdl2_k2_params &p) {
 	/* dynamic shared memory (K2_SMEM_BYTES): phase ring [160][BLOCK], staging area (modes 3 and 4), constants, unwrap table.
 	 * BLOCK = 128: the four warps of a block sit on the four sub-partitions of one SM, one each, exactly like K1's, so
 	 * that a K1 block and a K2 block always fit side by side (a 250-register warp takes half a sub-partition's register
@@ -1112,8 +1172,8 @@ __global__ void __launch_bounds__(BLOCK) k2_sync_slice(vdl2_k2_params p) {
 	const float2 *dec = p.dec + ch;
 	const float *phs = p.phase + (size_t)VDL2_SYNC_BUFLEN * s + ch;      /* row 0 of phs = first sample of this chunk */
 	const float *mgs = p.mag + ch;
-	const uint32_t n_dec = p.ca ? p.ca->n_dec : p.n_dec;
-	const uint64_t dec_base = p.ca ? p.ca->dec_base : p.dec_base;
+	const uint32_t n_dec = RAGGED ? p.rx_span[p.slot_rx[ch]].n : p.ca ? p.ca->n_dec : p.n_dec;
+	const uint64_t dec_base = RAGGED ? p.rx_span[p.slot_rx[ch]].dec_base : p.ca ? p.ca->dec_base : p.dec_base;
 	uint32_t m = 0;
 	if(BLOCKED) {
 		if(MODE == 4) {
@@ -1252,6 +1312,11 @@ __global__ void __launch_bounds__(BLOCK) k2_sync_slice(vdl2_k2_params p) {
 	st[K2_PURE_RUN * s + ch] = v.pure_run;
 	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);       /* thread 0's own end: an approximation of the block's */
 }
+
+template<int BLOCK, bool BLOCKED, int MODE>
+__global__ void __launch_bounds__(BLOCK) k2_sync_slice(vdl2_k2_params p) { k2_sync_body<BLOCK, BLOCKED, MODE, false>(p); }
+/* ragged spans: the default walk (mode 4) in 128-thread blocks */
+__global__ void __launch_bounds__(128) k2_sync_slice_ragged(vdl2_k2_params p) { k2_sync_body<128, true, 4, true>(p); }
 
 /* ------------------------------------------------------------------------------------------------
  * K3: one block per completed burst (grid-stride over the ready list).
@@ -1491,6 +1556,15 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		vdl2_set_carveout(k1_mix_iir_decimate_mixed<false>, pct);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_mixed<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_mixed<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
+		vdl2_set_carveout(k0_convert_ragged, pct);
+		vdl2_set_carveout(k1_mix_iir_decimate_ragged<true>, pct);
+		vdl2_set_carveout(k1_mix_iir_decimate_ragged<false>, pct);
+		cudaFuncSetAttribute(k1_mix_iir_decimate_ragged<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
+		cudaFuncSetAttribute(k1_mix_iir_decimate_ragged<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
+		vdl2_set_carveout(k2a_phase_mag_warps_ragged<true>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps_ragged<false>, pct);
+		vdl2_set_carveout(k2_sync_slice_ragged, pct);
+		cudaFuncSetAttribute(k2_sync_slice_ragged, cudaFuncAttributeMaxDynamicSharedMemorySize, K2_SMEM_BYTES(K2_BLOCK, 4));
 		vdl2_set_carveout(k2a_phase_mag<true>, pct);
 		vdl2_set_carveout(k2a_phase_mag_warps<true>, pct);
 		vdl2_set_carveout(k2a_phase_mag_warps<false>, pct);
@@ -1533,6 +1607,14 @@ extern "C" int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_
 	return (int)cudaGetLastError();
 }
 
+extern "C" int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
+		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st) {
+	if(width == 0 || n_rx == 0) return 0;
+	k0_convert_ragged<<<dim3((width * os_max + 255) / 256, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), rx, span, levels,
+			reinterpret_cast<float2 *>(out2), out_stride, ca);
+	return (int)cudaGetLastError();
+}
+
 template<int OS, int BLOCK>
 static void k1_launch_packed(const vdl2_k1_params *p, int variant, bool sym, cudaStream_t st) {
 	const uint32_t blocks = (p->n_chp + BLOCK - 1) / BLOCK;
@@ -1565,7 +1647,10 @@ extern "C" int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int var
 		bool msym = variant != 4;
 		for(int k = 0; k < 3; k++)
 			if(p->cls_mask & (1u << k)) msym = msym && p->cls_taps[k][1] == 2.0f * p->cls_taps[k][0] && p->cls_taps[k][2] == p->cls_taps[k][0];
-		if(msym) k1_mix_iir_decimate_mixed<true><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p);
+		if(p->rx_span) {                              /* ragged spans: n_pairs is the span's width */
+			if(msym) k1_mix_iir_decimate_ragged<true><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p);
+			else k1_mix_iir_decimate_ragged<false><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p);
+		} else if(msym) k1_mix_iir_decimate_mixed<true><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p);
 		else k1_mix_iir_decimate_mixed<false><<<blocks, VDL2_RX_K1_BLOCK, smem, st>>>(*p);
 		return (int)cudaGetLastError();
 	}
@@ -1620,7 +1705,10 @@ extern "C" int vdl2_launch_k2a(const vdl2_k2_params *p, cudaStream_t st) {
 extern "C" int vdl2_launch_k2a_warps(const vdl2_k2a_params *p, cudaStream_t st) {
 	if(p->n_ch == 0) return 0;
 	const uint32_t blocks = ((p->n_chp + 127u) / 128u) * (p->split ? p->split : 1u);
-	if(p->mode) k2a_phase_mag_warps<true><<<blocks, 128, 0, st>>>(*p);
+	if(p->rx_span) {                                  /* ragged spans */
+		if(p->mode) k2a_phase_mag_warps_ragged<true><<<blocks, 128, 0, st>>>(*p);
+		else k2a_phase_mag_warps_ragged<false><<<blocks, 128, 0, st>>>(*p);
+	} else if(p->mode) k2a_phase_mag_warps<true><<<blocks, 128, 0, st>>>(*p);
 	else k2a_phase_mag_warps<false><<<blocks, 128, 0, st>>>(*p);
 	return (int)cudaGetLastError();
 }
@@ -1631,6 +1719,10 @@ extern "C" int vdl2_launch_k2a_warps(const vdl2_k2a_params *p, cudaStream_t st) 
 extern "C" int vdl2_launch_k2(const vdl2_k2_params *p, cudaStream_t st) {
 	if(p->n_dec == 0 || p->n_ch == 0) return 0;
 	uint32_t blocks = (p->n_chp + K2_BLOCK - 1) / K2_BLOCK;
+	if(p->rx_span) {                              /* ragged spans: the default walk, whatever the variant */
+		k2_sync_slice_ragged<<<blocks, K2_BLOCK, K2_SMEM_BYTES(K2_BLOCK, 4), st>>>(*p);
+		return (int)cudaGetLastError();
+	}
 	const uint32_t variant = p->variant & 0xFFu;
 	if(p->variant & 0x100u) {                     /* A/B: one warp per block (VDL2GPU_K2_VARIANT = 256 + variant) */
 		blocks = (p->n_chp + 31u) / 32u;

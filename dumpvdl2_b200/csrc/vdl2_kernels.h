@@ -70,6 +70,9 @@ typedef struct {
 	const uint8_t *slot_cls;
 	float cls_taps[3][5];
 	uint32_t cls_mask, rx_os_max;
+	/* ragged spans (VDL2GPU_FLAG_RAGGED; NULL otherwise): the span's receiver table (vdl2_rx_span_table); receiver r's row
+	 * holds rx_span[r].n x os_r samples, and n_pairs (or ca->n_pairs) is the span's width, the largest n */
+	const vdl2_rx_span *rx_span;
 } vdl2_k1_params;
 
 typedef struct {
@@ -97,6 +100,9 @@ typedef struct {
 	uint32_t k2a_mode;           /* 0: libdevice atan2 for every sample; 1: vdl2_phase_fast with the Ziv fall-back */
 	const vdl2_chunk_args *ca;   /* NULL, or device pointer overriding n_dec / dec_base */
 	vdl2_block_trace *trace_blocks;
+	/* ragged spans (NULL otherwise): a lane walks rx_span[slot_rx[slot]].n samples from index rx_span[...].dec_base */
+	const uint32_t *slot_rx;
+	const vdl2_rx_span *rx_span;
 } vdl2_k2_params;
 
 /* K2a in its resident form (k2a_phase_mag_warps): warp w computes phase and magnitude of slots [32 w, 32 w + 32) for every
@@ -111,6 +117,10 @@ typedef struct {
 	uint32_t mode;               /* 0 libdevice atan2 / IEEE sqrt for every sample, 1 the Ziv-guarded short forms */
 	uint32_t split;              /* time slices per chunk: the grid is `split` x (one block per 128 slots) */
 	const vdl2_chunk_args *ca;
+	/* ragged spans (NULL otherwise): a lane's rows are rx_span[slot_rx[slot]].n, its history the previous plane's rows
+	 * [prev_n, prev_n + 160) */
+	const uint32_t *slot_rx;
+	const vdl2_rx_span *rx_span;
 } vdl2_k2a_params;
 
 typedef struct {
@@ -140,6 +150,10 @@ int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t fmt, const 
  * rx[r].off_per_dec into out2 + r x out_stride float2 (n_dec from ca->n_pairs when ca is given) */
 int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *rx, uint32_t n_rx, uint32_t os_max, const float *levels,
 		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
+/* ragged spans: row r converts span[r].n x rx[r].oversample samples from raw + span[r].off; width = the largest span[r].n
+ * (sizes the grid) */
+int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
+		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
 int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st);
 /* whether vdl2_launch_k1 with these arguments runs a kernel that honours p->phase (the pipelined packed kernel with
  * 128-channel blocks); everything else, the receiver-group kernel included, leaves the phase plane to K2a */

@@ -51,7 +51,9 @@ enum {
 	VDL2GPU_FLAG_KEEP_DEC = 1u << 1,     /* keep the decimated samples of the last chunk readable (parity tests) */
 	VDL2GPU_FLAG_K1_SCALAR = 1u << 2,    /* use the plain per-sample K1 kernel instead of the pipelined one */
 	VDL2GPU_FLAG_NO_OVERLAP = 1u << 3,   /* one stream: do not run K0/K1 of chunk c+1 beside K2/K3 of chunk c (profiling) */
-	VDL2GPU_FLAG_NO_GRAPH = 1u << 4      /* launch every kernel individually instead of replaying the per-chunk CUDA graphs */
+	VDL2GPU_FLAG_NO_GRAPH = 1u << 4,     /* launch every kernel individually instead of replaying the per-chunk CUDA graphs */
+	VDL2GPU_FLAG_RAGGED = 1u << 5        /* vdl2gpu_create_mixed_receivers only: every receiver brings its own number of decimated
+	                                      * samples to a span (vdl2gpu_submit_ragged); every other create function refuses it */
 };
 
 typedef struct {
@@ -98,8 +100,10 @@ typedef void (*vdl2gpu_frame_cb)(const vdl2gpu_frame *frame, void *user);
 /* per-context counters; names follow the reference's statsd counters (src/statsd.c:33-64) */
 typedef struct {
 	uint64_t chunks_submitted, chunks_completed;
-	uint64_t iq_samples;                 /* complex samples accepted (per stream; a mixed-receivers context: of all receivers) */
-	uint64_t dec_samples;                /* decimated samples produced per channel */
+	uint64_t iq_samples;                 /* complex samples accepted (per stream; a mixed-receivers context: of all receivers; ragged
+	                                      * spans: the complex samples actually submitted, sum over r of n_r x oversample_r) */
+	uint64_t dec_samples;                /* decimated samples produced per channel (ragged spans: the sum of the span widths, the
+	                                      * largest n_r of each span; vdl2gpu_get_receiver_positions has each receiver's count) */
 	uint64_t demod_sync_good;            /* demod.sync.good */
 	uint64_t decoder_crc_good;           /* decoder.crc.good (header syndrome 0) */
 	uint64_t bursts;                     /* bursts that reached DEC_DATA */
@@ -150,7 +154,9 @@ int vdl2gpu_create_receivers(const vdl2gpu_config *cfg, const vdl2gpu_receiver *
  * vdl2gpu_submit_planar_s16 return VDL2GPU_EINVAL).  max_chunk_bytes bounds the buffer of any one receiver in a span:
  * n_dec <= max_chunk_bytes / max over r of (oversample_r x bytes per complex sample_r).  vdl2gpu_get_tables returns
  * VDL2GPU_EINVAL (there is no single rate); stats.iq_samples counts the complex samples of all receivers.  Listing the
- * receivers grouped by rate keeps the 32 channels of a K1 warp on one rate, which runs faster than interleaved rates. */
+ * receivers grouped by rate keeps the 32 channels of a K1 warp on one rate, which runs faster than interleaved rates.
+ * With VDL2GPU_FLAG_RAGGED in cfg->flags the receivers do not advance in lock step: every receiver brings its own number
+ * of decimated samples to each span (vdl2gpu_submit_ragged); a uniform fleet gets ragged spans by describing itself here. */
 typedef struct {
 	uint32_t centerfreq;         /* Hz */
 	uint32_t n_channels;         /* >= 1; the next n_channels entries of cfg->freqs */
@@ -186,6 +192,25 @@ int vdl2gpu_submit_device(vdl2gpu_ctx *ctx, const void *dev_iq, uint32_t len, vo
  * Same buffer and stream rules as vdl2gpu_submit / vdl2gpu_submit_device. */
 int vdl2gpu_submit_span(vdl2gpu_ctx *ctx, const void *iq, uint32_t n_dec);
 int vdl2gpu_submit_span_device(vdl2gpu_ctx *ctx, const void *dev_iq, uint32_t n_dec, void *producer_stream);
+/* Ragged spans (a context made by vdl2gpu_create_mixed_receivers with VDL2GPU_FLAG_RAGGED): receiver r brings its own
+ * n_dec[r] >= 0 decimated samples to the span, i.e. n_dec[r] x oversample_r complex samples in its own format, and the
+ * counts may differ from receiver to receiver and from span to span (0 for any number of spans, fewer than 12 or 160, ...).
+ * Receivers need not be paced against each other: every receiver decodes exactly what one reference process at its rate
+ * decodes from the concatenation of everything that receiver brought, however the streams were cut.  The n_rx buffers lie
+ * back to back, receiver 0 first: receiver r's starts sum over q < r of n_dec[q] x oversample_q x bytes per complex
+ * sample_q bytes in (a 64-bit offset).  All counts 0 is a no-op; a count above the largest span max_chunk_bytes allows for
+ * that receiver returns VDL2GPU_ETOOBIG; on any other context these calls return VDL2GPU_EINVAL.  Same buffer and stream
+ * rules as vdl2gpu_submit_span / vdl2gpu_submit_span_device, which on a ragged context are these calls with all counts
+ * equal.  Frames' sync_dec_index, trace events' dec_index and burst timestamps count in the receiver's own decimated
+ * samples; a burst's timestamp is the span's arrival time moved back by the distance from its sync sample to the end of
+ * its receiver's samples in the span.  vdl2gpu_read_dec returns the span's width (largest count) in rows, of which only
+ * the first n_dec[r] are defined for the channels of receiver r. */
+int vdl2gpu_submit_ragged(vdl2gpu_ctx *ctx, const void *iq, const uint32_t *n_dec /* [n_rx] */);
+int vdl2gpu_submit_ragged_device(vdl2gpu_ctx *ctx, const void *dev_iq, const uint32_t *n_dec /* [n_rx], host memory */,
+		void *producer_stream);
+/* out[r] = decimated samples of receiver r accepted so far, for the first n_rx receivers of a receivers context (with ragged
+ * spans: the sum of receiver r's counts, which shows which receiver lags; in lock step all receivers are equal) */
+int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *ctx, uint64_t *out, uint32_t n_rx);
 int vdl2gpu_wait_input_consumed(vdl2gpu_ctx *ctx, void *stream);
 /* Make `stream` (cudaStream_t) wait for all device work enqueued by this context so far (for timing with
  * events recorded on the caller's stream, and for ordering consumers of device-side results). */
