@@ -85,6 +85,7 @@ def load_library():
     L.vdl2gpu_submit_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.vdl2gpu_submit_ragged_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.vdl2gpu_get_receiver_positions.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.vdl2gpu_restart_receiver.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
     L.vdl2gpu_destroy.argtypes = [C.c_void_p]
     L.vdl2gpu_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
@@ -410,7 +411,8 @@ class Vdl2MixedReceivers(Vdl2Receivers):
 
     With ragged=True the receivers do not advance in lock step: submit_ragged() takes whatever whole decimation groups each
     receiver has (any count, 0 included, per receiver and per span), and every receiver still decodes exactly what one
-    reference process decodes from the concatenation of its buffers."""
+    reference process decodes from the concatenation of its buffers.  restart_receiver() starts one receiver afresh (a
+    reconnect, a swapped device, a retune) without disturbing the others."""
 
     def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, ragged=False):
         """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16))"""
@@ -504,6 +506,26 @@ class Vdl2MixedReceivers(Vdl2Receivers):
         out = np.zeros(self.n_receivers, np.uint64)
         _check(self.L, self.L.vdl2gpu_get_receiver_positions(self.h, out.ctypes.data, self.n_receivers), "vdl2gpu_get_receiver_positions")
         return out
+
+    def restart_receiver(self, r, centerfreq=None, freqs=None):
+        """restart receiver r at the start of the next span that runs, as a freshly started reference process tuned to
+        centerfreq (None: its centre) and freqs (None: its channel frequencies; otherwise one per channel of the receiver);
+        every other receiver keeps its state.  receivers / freqs follow the new tuning."""
+        r = int(r)
+        if not 0 <= r < self.n_receivers:
+            raise ValueError(f"receiver {r} of {self.n_receivers}")
+        cf_old, fr_old = self.receivers[r]
+        fr = None
+        if freqs is not None:
+            fr = np.ascontiguousarray([int(f) for f in freqs], np.uint32)
+            if fr.size != len(fr_old):
+                raise ValueError(f"receiver {r} has {len(fr_old)} channels, {fr.size} frequencies given")
+        cf = 0 if centerfreq is None else int(centerfreq)
+        _check(self.L, self.L.vdl2gpu_restart_receiver(self.h, r, cf, fr.ctypes.data if fr is not None else None),
+               "vdl2gpu_restart_receiver")
+        new_fr = [int(f) for f in fr] if fr is not None else fr_old
+        self.receivers[r] = (cf if cf else cf_old, new_fr)
+        self.freqs[self._first[r]:self._first[r + 1]] = new_fr
 
     def process_ragged(self, bufs, counts_per_span):
         """each receiver's whole stream, cut into ragged spans: span k brings counts_per_span[k][r] decimated samples of

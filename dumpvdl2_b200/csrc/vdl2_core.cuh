@@ -1284,4 +1284,71 @@ VDL2_HD vdl2_rx_tile_row vdl2_rx_ragged_row(uint32_t n_r, uint32_t g0, uint32_t 
 	return t;
 }
 
+/* ------------------------------------------------------------------------------------------------
+ * Restarting one receiver of a ragged context (vdl2gpu_restart_receiver): from the start of a span on, its channels
+ * decode what a freshly started reference process, tuned to the receiver's (possibly new) centre and frequencies, decodes
+ * from the samples the receiver brings from then on.  One rule for create and restart, so the two cannot drift apart.
+ * ---------------------------------------------------------------------------------------------- */
+/* the NCO step of a channel (src/demod.c:385); a channel on the centre frequency skips the mixer in the reference
+ * (src/demod.c:312): with a zero step the table gives cos = 1, sin = 0 and the products are exact, so no branch is needed */
+VDL2_HD uint32_t vdl2_nco_dphi(uint32_t centerfreq, uint32_t freq, uint32_t rate) {
+	if(centerfreq == freq) return 0u;
+	return (uint32_t)(int)F_MUL(F_MUL(F_DIV(F_SUB((float)centerfreq, (float)freq), (float)rate), 256.0f), 65536.0f);
+}
+
+/* the K1 state of a freshly started channel in slot ch of the K1 planes: zero delay lines, NCO phase 0, the channel's step
+ * (the decimation counter is not per channel: it is 0 at the start of every span of a mixed-receivers context) */
+VDL2_HD void vdl2_k1_fresh(uint32_t *st, size_t stride, uint32_t ch, uint32_t dphi) {
+	for(int f = 0; f < K1_NFIELDS; f++) st[(size_t)f * stride + ch] = 0u;
+	st[(size_t)K1_DPHI * stride + ch] = dphi;
+}
+
+/* one channel's K2 state as the K2 planes hold it (field f of slot ch at st[f * stride + ch]) */
+VDL2_HD void vdl2_chan_store(const vdl2_chan &v, uint32_t *st, size_t stride, uint32_t ch) {
+	union { float f; uint32_t u; } b;
+#define VDL2_ST_F(F, X) do { b.f = (X); st[(size_t)(F) * stride + ch] = b.u; } while(0)
+	VDL2_ST_F(K2_PREV_PHI, v.prev_phi); VDL2_ST_F(K2_PREV_DPHI, v.prev_dphi); VDL2_ST_F(K2_DPHI, v.dphi);
+	VDL2_ST_F(K2_PHERR0, v.pherr0); VDL2_ST_F(K2_PHERR1, v.pherr1); VDL2_ST_F(K2_PHERR2, v.pherr2);
+	VDL2_ST_F(K2_PPM, v.ppm_error); VDL2_ST_F(K2_MAG_LP, v.mag_lp); VDL2_ST_F(K2_MAG_NF, v.mag_nf);
+	VDL2_ST_F(K2_FRAME_PWR, v.frame_pwr);
+#undef VDL2_ST_F
+	st[(size_t)K2_RING_POS * stride + ch] = (uint32_t)v.ring_pos; st[(size_t)K2_SCLK * stride + ch] = (uint32_t)v.sclk;
+	st[(size_t)K2_NFCNT * stride + ch] = (uint32_t)v.nfcnt; st[(size_t)K2_FRAME_PWR_CNT * stride + ch] = (uint32_t)v.frame_pwr_cnt;
+	st[(size_t)K2_STATE * stride + ch] = v.state;
+	st[(size_t)K2_ACC_LO * stride + ch] = (uint32_t)v.acc; st[(size_t)K2_ACC_HI * stride + ch] = (uint32_t)(v.acc >> 32);
+	st[(size_t)K2_NBITS * stride + ch] = v.nbits; st[(size_t)K2_NEED_BITS * stride + ch] = v.need_bits;
+	st[(size_t)K2_DATALEN * stride + ch] = v.datalen; st[(size_t)K2_SYNDROME * stride + ch] = v.syndrome;
+	st[(size_t)K2_SLOT * stride + ch] = (uint32_t)v.slot; st[(size_t)K2_BURST_SEQ * stride + ch] = v.burst_seq;
+	st[(size_t)K2_SYNC_LO * stride + ch] = (uint32_t)v.sync_dec_index; st[(size_t)K2_SYNC_HI * stride + ch] = (uint32_t)(v.sync_dec_index >> 32);
+	st[(size_t)K2_FREQ * stride + ch] = v.freq;
+	st[(size_t)K2_CNT_SYNC * stride + ch] = v.cnt_sync; st[(size_t)K2_CNT_HDR_GOOD * stride + ch] = v.cnt_hdr_good;
+	st[(size_t)K2_PURE_RUN * stride + ch] = v.pure_run;
+}
+
+/* a ready-list entry with this bit set is a burst-pool slot given up by a restart, not a burst: K3 puts it back on the
+ * free list and writes no record, counts nothing, emits nothing */
+#define VDL2_READY_ABANDONED 0x80000000u
+
+/* Restart of one channel's demodulator: the old process is treated as killed here.  A burst still in progress (header
+ * decoded, data being collected) is dropped; the burst-pool slot it holds goes back to the pool through K3 (ready list,
+ * VDL2_READY_ABANDONED): other lanes pop the free list concurrently, so pushing onto it from here would race them.
+ * Every field is then as vdl2_chan_init leaves it, tuned to `freq`, except the burst sequence number and the two
+ * per-channel counters kept in the state: they continue, so that (channel, burst_seq, idx) never repeats and the
+ * counters are the sum over the old and the new process.  The caller zeroes the channel's syncbuf ring. */
+VDL2_HD void vdl2_chan_restart(vdl2_chan &v, const vdl2_k2_env &env, uint32_t freq) {
+	if(v.slot >= 0) {
+		const uint32_t k = VDL2_ATOMIC_ADD_U32(&env.ctl->n_ready, 1u);
+		env.ready[k] = (uint32_t)v.slot | VDL2_READY_ABANDONED;
+	}
+	const uint32_t seq = v.burst_seq, cnt_sync = v.cnt_sync, cnt_hdr_good = v.cnt_hdr_good;
+	vdl2_chan_init(v, freq);
+	v.burst_seq = seq; v.cnt_sync = cnt_sync; v.cnt_hdr_good = cnt_hdr_good;
+}
+
+/* one channel slot's entry of a span's restart table: restart != 0 = the channel restarts at the start of the span with K1
+ * step dphi (vdl2_nco_dphi) and frequency freq */
+typedef struct {
+	uint32_t restart, dphi, freq;
+} vdl2_rx_restart;
+
 #endif

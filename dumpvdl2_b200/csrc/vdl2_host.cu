@@ -59,6 +59,11 @@ struct chunk_slot {
 	vdl2_chunk_args *h_args = nullptr, *d_args = nullptr;
 	/* ragged spans: the span's receiver table (vdl2_rx_span_table; pinned host copy, device copy made with the arguments) */
 	vdl2_rx_span *h_span = nullptr, *d_span = nullptr;
+	/* ragged spans that restart receivers (vdl2gpu_restart_receiver): per channel slot, whether it starts afresh with this
+	 * span and its new tuning (pinned host copy, device copy made with the span's table); such a span takes the direct
+	 * path, so the graphs of ordinary spans never see the table */
+	vdl2_rx_restart *h_restart = nullptr, *d_restart = nullptr;
+	bool restart = false;
 	cudaGraphExec_t g_front[6] = { nullptr }, g_k2a[6] = { nullptr }, g_back[6] = { nullptr };    /* index = chunk number mod 6 (dec buffer, plane) */
 	uint32_t graph_pairs[6] = { 0 };
 	uint64_t first_pair = 0, dec_base = 0;
@@ -107,6 +112,11 @@ struct vdl2gpu_ctx {
 	std::vector<uint64_t> rx_pos;                       /* per receiver: decimated samples accepted so far */
 	std::vector<uint32_t> rx_prev;                      /* per receiver: its count in the previous span */
 	std::vector<uint32_t> ch_rx;                        /* per channel: its receiver (burst timestamps) */
+	/* restarts (vdl2gpu_restart_receiver): every receiver's current centre and first channel, and the receivers whose
+	 * restart waits for the next span that runs */
+	std::vector<uint32_t> rx_centre, rx_first;
+	std::vector<uint8_t> rx_restart_pending;
+	uint32_t n_restart_pending = 0;
 	uint32_t raw_bytes = 0;                             /* size of each slot's raw staging buffers (allocated on the first host submit) */
 	int k1_variant = 2, k2_variant = 5, k2a_mode = 1;   /* A/B knobs (VDL2GPU_K1_VARIANT, VDL2GPU_K2_VARIANT, VDL2GPU_K2A), read at create */
 	bool use_graphs = true;
@@ -146,10 +156,6 @@ struct vdl2gpu_ctx {
 	std::vector<std::vector<uint8_t>> blobs;
 	cudaEvent_t ev_drain = nullptr;
 };
-
-static uint32_t dphi_for(uint32_t centerfreq, uint32_t freq, uint32_t rate) {      /* src/demod.c:385 */
-	return (uint32_t)(int)(((float)centerfreq - (float)freq) / (float)rate * 256.0f * 65536.0f);
-}
 
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
 		uint32_t n_chp, uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2);
@@ -205,6 +211,8 @@ static int free_ctx(vdl2gpu_ctx *c) {
 		if(s.d_args) cudaFree(s.d_args);
 		if(s.h_span) cudaFreeHost(s.h_span);
 		if(s.d_span) cudaFree(s.d_span);
+		if(s.h_restart) cudaFreeHost(s.h_restart);
+		if(s.d_restart) cudaFree(s.d_restart);
 	}
 	cudaFree(c->d_tab); cudaFree(c->d_samples);
 	for(int i = 0; i < 3; i++) cudaFree(c->d_dec3[i]);
@@ -440,6 +448,10 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 			c->rx_prev.assign(n_rx, 0);
 			c->ch_rx.resize(c->n_ch);
 			for(uint32_t r = 0; r < n_rx; r++) std::fill(c->ch_rx.begin() + rx_first[r], c->ch_rx.begin() + rx_first[r + 1], r);
+			c->rx_first = rx_first;
+			c->rx_centre.resize(n_rx);
+			for(uint32_t r = 0; r < n_rx; r++) c->rx_centre[r] = rx[r].centerfreq;
+			c->rx_restart_pending.assign(n_rx, 0);
 		}
 	}
 	initial_state(c->cfg, c->freqs.data(), c->receivers ? centres.data() : nullptr, c->mixed ? rates.data() : nullptr, c->n_ch, c->n_chp,
@@ -463,6 +475,8 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 		if(c->ragged) {
 			CU(cudaHostAlloc((void **)&s.h_span, (size_t)n_rx * sizeof(vdl2_rx_span), cudaHostAllocDefault));
 			CU(cudaMalloc(&s.d_span, (size_t)n_rx * sizeof(vdl2_rx_span)));
+			CU(cudaHostAlloc((void **)&s.h_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart), cudaHostAllocDefault));
+			CU(cudaMalloc(&s.d_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart)));
 		}
 		CU(cudaHostAlloc((void **)&s.h_out, sizeof(vdl2_out_header) + c->out_cap, cudaHostAllocMapped));
 		CU(cudaHostGetDevicePointer((void **)&s.d_out, s.h_out, 0));
@@ -752,8 +766,11 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	p2.events = c->d_events; p2.event_cap = c->event_cap; p2.trace = (c->cfg.flags & VDL2GPU_FLAG_TRACE) ? 1u : 0u;
 	p2.variant = (uint32_t)c->k2_variant; p2.k2a_mode = (uint32_t)c->k2a_mode; p2.ca = ca;
 	p1.rx_span = s.d_span; pa.slot_rx = c->d_slot_rx; pa.rx_span = s.d_span; p2.slot_rx = c->d_slot_rx; p2.rx_span = s.d_span;   /* (NULL unless ragged) */
+	/* the restart table only on a span that restarts receivers, which is never captured (NULL in every graph) */
+	const vdl2_rx_restart *rs = (s.restart && !ca) ? s.d_restart : nullptr;
+	p1.rx_restart = rs; pa.rx_restart = rs; p2.rx_restart = rs;
 	p3.pool = c->d_pool; p3.free_list = c->d_free; p3.ready = c->d_ready; p3.ctl = c->d_ctl; p3.tables = c->d_tab;
-	p3.out = s.d_out; p3.out_cap = c->out_cap; p3.n_chp = c->n_chp; p3.counters = c->d_counters;
+	p3.out = s.d_out; p3.out_cap = c->out_cap; p3.n_chp = c->n_chp; p3.counters = c->d_counters; p3.abandoned = rs ? 1u : 0u;
 }
 
 #define K3_GRID (132u * 16u)      /* 16 resident blocks on each of the 132 SMs of an H100: ~1.7 bursts per block per chunk at the bench traffic */
@@ -861,6 +878,7 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	bool graph = c->use_graphs && !planar && overlap;
 	if(graph && c->graph_nominal == 0) c->graph_nominal = n_pairs;
 	graph = graph && n_pairs == c->graph_nominal;            /* odd-sized chunks (the tail of a file) take the direct path */
+	graph = graph && !s.restart;                             /* ... and so do spans that restart receivers */
 	if(graph && ensure_graphs(c, s, seq, n_pairs, k0_fmt) != VDL2GPU_OK) { c->use_graphs = false; graph = false; }
 	vdl2_k1_params p1; vdl2_k2a_params pa; vdl2_k2_params p2; vdl2_k3_params p3;
 	fill_params(c, s, seq, n_pairs, c->decim_cnt, s.n_dec, c->last_n_dec, s.dec_base, nullptr, p1, pa, p2, p3);
@@ -884,6 +902,7 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 		CU(cudaGraphLaunch(s.g_front[gk], c->stream));
 	} else {
 		if(c->ragged) CU(cudaMemcpyAsync(s.d_span, s.h_span, c->n_streams * sizeof(vdl2_rx_span), cudaMemcpyHostToDevice, c->stream));
+		if(s.restart) CU(cudaMemcpyAsync(s.d_restart, s.h_restart, c->n_chp * sizeof(vdl2_rx_restart), cudaMemcpyHostToDevice, c->stream));
 		if(c->mixed) { int rc = launch_k0_span(c, s, d_raw, n_pairs, nullptr); if(rc) return rc; }
 		else if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 				n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, nullptr, c->stream));
@@ -1067,6 +1086,26 @@ static int span_check(vdl2gpu_ctx *c, const void *iq, uint32_t n_dec, const char
 	return 0;
 }
 
+/* the restart table of the span about to run in slot s (its previous chunk has been harvested): every receiver with a
+ * restart pending restarts at the start of this span, with its current tuning */
+static void fill_restarts(vdl2gpu_ctx *c, chunk_slot &s) {
+	s.restart = c->n_restart_pending != 0;
+	if(!s.restart) return;
+	memset(s.h_restart, 0, (size_t)c->n_chp * sizeof(vdl2_rx_restart));
+	for(uint32_t r = 0; r < c->n_streams; r++) {
+		if(!c->rx_restart_pending[r]) continue;
+		const uint32_t rate = (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * c->rx_in[r].oversample;
+		for(uint32_t chan = c->rx_first[r]; chan < c->rx_first[r + 1]; chan++) {
+			vdl2_rx_restart &e = s.h_restart[slot_of(chan, c->lanes, c->full_warps)];
+			e.restart = 1u;
+			e.dphi = vdl2_nco_dphi(c->rx_centre[r], c->freqs[chan], rate);
+			e.freq = c->freqs[chan];
+		}
+		c->rx_restart_pending[r] = 0;
+	}
+	c->n_restart_pending = 0;
+}
+
 /* Ragged spans: receiver r brings n_dec[r] decimated samples (host buffer, or device buffer ordered after producer_stream).
  * Everything is checked before the device is touched; the span then runs the chain at its width, the largest count, with
  * the span's receiver table (built in the slot's pinned copy: the slot's previous chunk has been harvested) telling every
@@ -1098,6 +1137,7 @@ static int ragged_submit(vdl2gpu_ctx *c, const void *iq, const uint32_t *n_dec, 
 	/* every buffer is at most max_span x its receiver's bytes per decimated sample <= max_chunk_bytes: the span fits the
 	 * max_chunk_bytes x n_rx staging buffer */
 	const uint64_t bytes = vdl2_rx_span_table(c->rx_in.data(), c->n_streams, n_dec, c->rx_pos.data(), c->rx_prev.data(), s->h_span);
+	fill_restarts(c, *s);
 	if(device) {
 		CU(cudaEventRecord(c->ev_input_ready, (cudaStream_t)producer_stream));
 		CU(cudaStreamWaitEvent(c->stream, c->ev_input_ready, 0));
@@ -1114,6 +1154,27 @@ extern "C" int vdl2gpu_submit_ragged(vdl2gpu_ctx *c, const void *iq, const uint3
 
 extern "C" int vdl2gpu_submit_ragged_device(vdl2gpu_ctx *c, const void *dev_iq, const uint32_t *n_dec, void *producer_stream) {
 	return ragged_submit(c, dev_iq, n_dec, true, producer_stream, "vdl2gpu_submit_ragged_device");
+}
+
+/* Restart receiver r at the start of the next span that runs (see include/vdl2gpu.h).  Only the host's record of the
+ * receiver's tuning changes here; the kernels of that span apply the restart, each at its own stage of the pipeline. */
+extern "C" int vdl2gpu_restart_receiver(vdl2gpu_ctx *c, uint32_t r, uint32_t centerfreq, const uint32_t *freqs) {
+	if(!c) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_restart_receiver: no context");
+		return VDL2GPU_EINVAL;
+	}
+	if(!c->ragged) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_restart_receiver: needs a context made by vdl2gpu_create_mixed_receivers with VDL2GPU_FLAG_RAGGED");
+		return VDL2GPU_EINVAL;
+	}
+	if(r >= c->n_streams) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_restart_receiver: receiver %u of %u", r, c->n_streams);
+		return VDL2GPU_EINVAL;
+	}
+	if(centerfreq) c->rx_centre[r] = centerfreq;
+	if(freqs) std::copy(freqs, freqs + (c->rx_first[r + 1] - c->rx_first[r]), c->freqs.begin() + c->rx_first[r]);
+	if(!c->rx_restart_pending[r]) { c->rx_restart_pending[r] = 1; c->n_restart_pending++; }
+	return VDL2GPU_OK;
 }
 
 extern "C" int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *c, uint64_t *out, uint32_t n_rx) {
@@ -1495,22 +1556,15 @@ extern "C" uint32_t vdl2gpu_stage_row_stride(uint32_t n_channels) { return (n_ch
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
 		uint32_t n_chp, uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2) {
 	k1.assign((size_t)K1_NFIELDS * n_chp, 0u); k2.assign((size_t)K2_NFIELDS * n_chp, 0u);
-	auto fbits = [](float f) { uint32_t u; memcpy(&u, &f, 4); return u; };
 	for(uint32_t chan = 0; chan < n_ch; chan++) {
 		const uint32_t ch = slot_of(chan, lanes, full_warps);          /* index into the per-channel planes */
-		/* a channel on the centre frequency skips the mixer in the reference (src/demod.c:312); with a zero
-		 * phase step the table gives cos = 1, sin = 0 and the products are exact, so no branch is needed */
 		const uint32_t centre = centres ? centres[chan] : cfg.centerfreq;     /* centres: per channel, multi-receiver context */
 		const uint32_t rate = rates ? rates[chan] : cfg.sample_rate;          /* rates: per channel, mixed-rate receivers */
-		k1[(size_t)K1_DPHI * n_chp + ch] = (centre != freqs[chan]) ? dphi_for(centre, freqs[chan], rate) : 0u;
-		k2[(size_t)K2_MAG_NF * n_chp + ch] = fbits(2.0f);
-		k2[(size_t)K2_PHERR1 * n_chp + ch] = fbits(1000.f);
-		k2[(size_t)K2_PHERR2 * n_chp + ch] = fbits(1000.f);
-		k2[(size_t)K2_STATE * n_chp + ch] = VDL2_DEC_HEADER << VDL2_DEC_SHIFT;
-		k2[(size_t)K2_NEED_BITS * n_chp + ch] = VDL2_HEADER_LEN;
-		k2[(size_t)K2_SLOT * n_chp + ch] = (uint32_t)-1;
-		k2[(size_t)K2_FREQ * n_chp + ch] = freqs[chan];
-		k2[(size_t)K2_PURE_RUN * n_chp + ch] = 0x40000000u;      /* VDL2_PURE_SATURATED: ring of zeros == history of zeros */
+		/* the same fresh state a restart gives (vdl2_core.cuh; the ring of zeros is the cudaMemset of create) */
+		vdl2_k1_fresh(k1.data(), n_chp, ch, vdl2_nco_dphi(centre, freqs[chan], rate));
+		vdl2_chan v;
+		vdl2_chan_init(v, freqs[chan]);
+		vdl2_chan_store(v, k2.data(), n_chp, ch);
 	}
 }
 

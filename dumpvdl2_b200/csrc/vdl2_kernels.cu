@@ -863,7 +863,10 @@ __device__ __forceinline__ uint32_t k1r_block_width(const vdl2_rx_span *span, ui
  * across the block and runs to the largest count of the block's receivers, which each warp reduces for itself at the
  * start (no shared slot, no extra barrier).  Row r of the tile at group g0 stages vdl2_rx_ragged_row(n_r, g0, ...): a row
  * with nothing left issues no copy, and the tile's expected transaction bytes are the sum of the copies issued.  A lane
- * runs the groups its receiver has in the tile; a lane whose receiver brought nothing neither loads nor stores its state. */
+ * runs the groups its receiver has in the tile; a lane whose receiver brought nothing neither loads nor stores its state.
+ * A lane whose channel restarts with this span (p.rx_restart non-NULL and its entry set) starts from the fresh state of
+ * vdl2_k1_fresh instead of the stored one - zero delay lines, NCO phase 0, the new step - and stores it even when its
+ * receiver brings nothing, or no receiver of the block does, so that the next span starts from it. */
 template<bool SYM, bool RAGGED>
 __device__ __forceinline__ void k1_mixed_body(const vdl2_k1_params &p) {
 	constexpr int NLUT = 8;
@@ -877,7 +880,9 @@ __device__ __forceinline__ void k1_mixed_body(const vdl2_k1_params &p) {
 	const int trace_k = tid == 0 ? vdl2_trace_begin(p.trace_blocks, 1) : -1;
 	const uint32_t ch = blockIdx.x * VDL2_RX_K1_BLOCK + tid;
 	uint32_t chan;
-	const bool active = vdl2_slot_channel(ch, p.lanes, p.full_warps, p.n_ch, chan) && (!RAGGED || p.rx_span[p.slot_rx[ch]].n > 0);
+	const bool live = vdl2_slot_channel(ch, p.lanes, p.full_warps, p.n_ch, chan);
+	const bool fresh = RAGGED && live && p.rx_restart != nullptr && p.rx_restart[ch].restart != 0u;
+	const bool active = live && (!RAGGED || p.rx_span[p.slot_rx[ch]].n > 0);
 	const uint32_t row = p.slot_rx[ch] - rx0;                                /* this lane's receiver within the block */
 	const uint32_t cls = p.slot_cls[ch];                                     /* ... and its rate class */
 	/* decimated samples per receiver (ragged: the most any receiver of the block brings) */
@@ -890,7 +895,8 @@ __device__ __forceinline__ void k1_mixed_body(const vdl2_k1_params &p) {
 	if(tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
 	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
 	uint32_t phi = 0, dphi = 0;
-	if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
+	if(RAGGED && fresh) dphi = p.rx_restart[ch].dphi;                         /* (the other fields stay 0) */
+	else if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
 	u64 x1 = f2_pack(xr1, xi1), x2 = f2_pack(xr2, xi2), y1 = f2_pack(yr1, yi1), y2 = f2_pack(yr2, yi2);
 	auto tap = [&](int j) { return cls == 0 ? p.cls_taps[0][j] : cls == 1 ? p.cls_taps[1][j] : p.cls_taps[2][j]; };
 	const float a0 = tap(0), a1 = tap(1), a2 = tap(2), b1 = tap(3), b2 = tap(4);
@@ -938,7 +944,9 @@ __device__ __forceinline__ void k1_mixed_body(const vdl2_k1_params &p) {
 		__syncthreads();                                           /* every warp is done with this buffer */
 		if(tid < 32 && tile + 2 < n_tiles) request_tile(tile + 2, tile & 1u);
 	}
-	if(active) k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+	if(active || (RAGGED && fresh))
+		k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+	if(RAGGED && fresh) p.state[K1_DPHI * p.n_chp + ch] = dphi;
 	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);
 }
 
@@ -1003,7 +1011,8 @@ __global__ void __launch_bounds__(256) k2a_phase_mag(const float2 *__restrict__ 
  * That is the last 160 phases of the receiver's stream whatever prev_n is: the previous plane holds, per slot, the 160
  * history rows it was given followed by that slot's prev_n new rows.  With prev_n = 0 (the receiver brought nothing last
  * span) the range is the previous plane's own history rows, which are the right ones; with 0 < prev_n < 160 it straddles
- * history and new rows, still in order.  So the two alternating planes need no change for ragged spans. */
+ * history and new rows, still in order.  So the two alternating planes need no change for ragged spans.  A lane whose
+ * channel restarts with the span (p.rx_restart) writes zero history rows instead: the new process has no past. */
 template<bool FAST, bool RAGGED>
 __device__ __forceinline__ void k2a_warps_body(const vdl2_k2a_params &p) {
 	__shared__ double s_atan[VDL2_ATAN_TABLE_DOUBLES];
@@ -1025,8 +1034,15 @@ __device__ __forceinline__ void k2a_warps_body(const vdl2_k2a_params &p) {
 	if(slice == 0) {
 		const float *src = p.phase_prev + (size_t)prev_n_dec * s + slot;
 		float *dst = p.phase + slot;
+		if(RAGGED && p.rx_restart != nullptr && p.rx_restart[slot].restart != 0u) {
+			/* the channel restarts with this span: zero history rows, as create's cudaMemset leaves them (also with n = 0:
+			 * the next span takes this plane's rows [0, 160) as its history) */
 #pragma unroll 8
-		for(uint32_t i = 0; i < VDL2_SYNC_BUFLEN; i++) dst[(size_t)i * s] = src[(size_t)i * s];
+			for(uint32_t i = 0; i < VDL2_SYNC_BUFLEN; i++) dst[(size_t)i * s] = 0.f;
+		} else {
+#pragma unroll 8
+			for(uint32_t i = 0; i < VDL2_SYNC_BUFLEN; i++) dst[(size_t)i * s] = src[(size_t)i * s];
+		}
 	}
 	const float2 *dec = p.dec + slot;
 	float *ph = p.phase + (size_t)VDL2_SYNC_BUFLEN * s + slot, *mg = p.mag + slot;
@@ -1118,7 +1134,8 @@ __device__ __forceinline__ void k2_cp_async_wait_all() { asm volatile("cp.async.
  * from rx_span[r].dec_base, i.e. in the receiver's own decimated samples.  Legal because after the barrier that loads the
  * constants there is no block-wide barrier left, the cp.async staging copies each thread's own column, and the walk
  * functions of vdl2_core.cuh use no warp-synchronous intrinsics: each lane's loop bound is its own.  A lane whose receiver
- * brought nothing loads and stores its state unchanged. */
+ * brought nothing loads and stores its state unchanged, unless its channel restarts with the span: then it stores the
+ * fresh state. */
 template<int BLOCK, bool BLOCKED, int MODE, bool RAGGED>
 __device__ __forceinline__ void k2_sync_body(const vdl2_k2_params &p) {
 	/* dynamic shared memory (K2_SMEM_BYTES): phase ring [160][BLOCK], staging area (modes 3 and 4), constants, unwrap table.
@@ -1160,14 +1177,19 @@ __device__ __forceinline__ void k2_sync_body(const vdl2_k2_params &p) {
 	v.cnt_sync = st[K2_CNT_SYNC * s + ch]; v.cnt_hdr_good = st[K2_CNT_HDR_GOOD * s + ch];
 	v.pure_run = st[K2_PURE_RUN * s + ch];
 	float *ring = &s_ring[tid];
+	/* RAGGED: a channel that restarts with this span (p.rx_restart) starts from a zero syncbuf ring, as create leaves it */
+	const bool fresh = RAGGED && p.rx_restart != nullptr && p.rx_restart[ch].restart != 0u;
 #pragma unroll 4
-	for(int i = 0; i < VDL2_SYNC_BUFLEN; i++) ring[i * BLOCK] = p.ring[(size_t)i * s + ch];
+	for(int i = 0; i < VDL2_SYNC_BUFLEN; i++) ring[i * BLOCK] = fresh ? 0.f : p.ring[(size_t)i * s + ch];
 
 	vdl2_k2_env env;
 	env.pr_phase = s_consts; env.lr_X = s_consts + 16; env.lr_denom = s_consts[32];
 	env.max_ppm = p.max_ppm; env.s27 = p.s27; env.unwrap_lut = s_unwrap;
 	env.pool = p.pool; env.free_list = p.free_list; env.ready = p.ready; env.ctl = p.ctl;
 	env.events = reinterpret_cast<vdl2_event_rec *>(p.events); env.event_cap = p.event_cap; env.trace = p.trace;
+	/* ... and from the fresh demodulator state on its new frequency; a burst in progress is dropped, its pool slot handed
+	 * to K3 to put back (vdl2_chan_restart) */
+	if(fresh) vdl2_chan_restart(v, env, p.rx_restart[ch].freq);
 
 	const float2 *dec = p.dec + ch;
 	const float *phs = p.phase + (size_t)VDL2_SYNC_BUFLEN * s + ch;      /* row 0 of phs = first sample of this chunk */
@@ -1310,6 +1332,7 @@ __device__ __forceinline__ void k2_sync_body(const vdl2_k2_params &p) {
 	st[K2_SYNC_LO * s + ch] = (uint32_t)v.sync_dec_index; st[K2_SYNC_HI * s + ch] = (uint32_t)(v.sync_dec_index >> 32);
 	st[K2_CNT_SYNC * s + ch] = v.cnt_sync; st[K2_CNT_HDR_GOOD * s + ch] = v.cnt_hdr_good;
 	st[K2_PURE_RUN * s + ch] = v.pure_run;
+	if(fresh) st[K2_FREQ * s + ch] = v.freq;                    /* (the only span in which a channel's frequency changes) */
 	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);       /* thread 0's own end: an approximation of the block's */
 }
 
@@ -1356,7 +1379,11 @@ __device__ __forceinline__ int k3_rs_block(uint8_t *data, int fec_octets, const 
 	return count;
 }
 
-__global__ void __launch_bounds__(K3_BLOCK) k3_burst_fec(vdl2_k3_params p) {
+/* ABANDONED (k3_burst_fec_abandoned, spans that restart receivers only): an entry of the ready list marked
+ * VDL2_READY_ABANDONED is a burst-pool slot a restarted channel gave up mid-burst (vdl2_chan_restart); it goes back on the
+ * free list, with no record, no counter and no event */
+template<bool ABANDONED>
+__device__ __forceinline__ void k3_body(const vdl2_k3_params &p) {
 	__shared__ vdl2_burst_work w;
 	__shared__ uint8_t s_gexp[512];
 	__shared__ uint8_t s_glog[256];
@@ -1377,6 +1404,13 @@ __global__ void __launch_bounds__(K3_BLOCK) k3_burst_fec(vdl2_k3_params p) {
 	for(uint32_t b = blockIdx.x; b < n_ready; b += gridDim.x) {
 		__syncthreads();
 		const uint32_t slot_idx = p.ready[b];
+		if(ABANDONED && (slot_idx & VDL2_READY_ABANDONED)) {      /* (the whole block: the loop begins with a barrier) */
+			if(tid == 0) {
+				int32_t top = atomicAdd(&p.ctl->free_top, 1);
+				p.free_list[top] = (int32_t)(slot_idx & ~VDL2_READY_ABANDONED);
+			}
+			continue;
+		}
 		const vdl2_burst_slot *slot = &p.pool[slot_idx];
 		if(tid == 0) vdl2_burst_geometry(w, slot->datalen_bits, slot->nbits);
 		for(uint32_t i = tid; i < VDL2_MAX_BLOCKS * 256 / 4; i += K3_BLOCK) reinterpret_cast<uint32_t *>(w.tab)[i] = 0;
@@ -1463,6 +1497,9 @@ __global__ void __launch_bounds__(K3_BLOCK) k3_burst_fec(vdl2_k3_params p) {
 		}
 	}
 }
+
+__global__ void __launch_bounds__(K3_BLOCK) k3_burst_fec(vdl2_k3_params p) { k3_body<false>(p); }
+__global__ void __launch_bounds__(K3_BLOCK) k3_burst_fec_abandoned(vdl2_k3_params p) { k3_body<true>(p); }
 
 /* publish the chunk's totals into the mapped region and re-arm the queues for the next chunk */
 __global__ void k_chunk_finish(vdl2_k3_params p) {
@@ -1578,6 +1615,7 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		vdl2_set_carveout(k_copy_rows, pct);
 		vdl2_set_carveout(k_copy_hist, pct);
 		vdl2_set_carveout(k3_burst_fec, pct);
+		vdl2_set_carveout(k3_burst_fec_abandoned, pct);
 		vdl2_set_carveout(k_chunk_finish, pct);
 	});
 	return (int)cudaGetLastError();
@@ -1755,7 +1793,8 @@ extern "C" int vdl2_launch_copy_hist(const vdl2_k2_params *p, cudaStream_t st) {
 }
 
 extern "C" int vdl2_launch_k3(const vdl2_k3_params *p, uint32_t grid, cudaStream_t st) {
-	k3_burst_fec<<<grid, K3_BLOCK, 0, st>>>(*p);
+	if(p->abandoned) k3_burst_fec_abandoned<<<grid, K3_BLOCK, 0, st>>>(*p);     /* spans that restart receivers */
+	else k3_burst_fec<<<grid, K3_BLOCK, 0, st>>>(*p);
 	int e = (int)cudaGetLastError();
 	if(e) return e;
 	k_chunk_finish<<<1, 1, 0, st>>>(*p);

@@ -73,6 +73,9 @@ typedef struct {
 	/* ragged spans (VDL2GPU_FLAG_RAGGED; NULL otherwise): the span's receiver table (vdl2_rx_span_table); receiver r's row
 	 * holds rx_span[r].n x os_r samples, and n_pairs (or ca->n_pairs) is the span's width, the largest n */
 	const vdl2_rx_span *rx_span;
+	/* ragged spans that restart receivers (vdl2gpu_restart_receiver; NULL on every other span): per slot, whether its
+	 * channel starts afresh with this span and its new NCO step (vdl2_rx_restart) */
+	const vdl2_rx_restart *rx_restart;
 } vdl2_k1_params;
 
 typedef struct {
@@ -103,6 +106,8 @@ typedef struct {
 	/* ragged spans (NULL otherwise): a lane walks rx_span[slot_rx[slot]].n samples from index rx_span[...].dec_base */
 	const uint32_t *slot_rx;
 	const vdl2_rx_span *rx_span;
+	/* (NULL unless the span restarts receivers) per slot: start the demodulator afresh on frequency rx_restart[slot].freq */
+	const vdl2_rx_restart *rx_restart;
 } vdl2_k2_params;
 
 /* K2a in its resident form (k2a_phase_mag_warps): warp w computes phase and magnitude of slots [32 w, 32 w + 32) for every
@@ -121,6 +126,8 @@ typedef struct {
 	 * [prev_n, prev_n + 160) */
 	const uint32_t *slot_rx;
 	const vdl2_rx_span *rx_span;
+	/* (NULL unless the span restarts receivers) per slot: zero history rows instead of the previous plane's */
+	const vdl2_rx_restart *rx_restart;
 } vdl2_k2a_params;
 
 typedef struct {
@@ -133,6 +140,7 @@ typedef struct {
 	uint32_t out_cap;            /* bytes available for records */
 	uint32_t n_chp;
 	uint32_t *counters;          /* [VDL2_NUM_COUNTERS][n_chp] */
+	uint32_t abandoned;          /* the ready list may hold slots given up by a restart (VDL2_READY_ABANDONED) */
 } vdl2_k3_params;
 
 #ifdef __cplusplus

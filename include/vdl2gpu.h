@@ -211,6 +211,23 @@ int vdl2gpu_submit_ragged_device(vdl2gpu_ctx *ctx, const void *dev_iq, const uin
 /* out[r] = decimated samples of receiver r accepted so far, for the first n_rx receivers of a receivers context (with ragged
  * spans: the sum of receiver r's counts, which shows which receiver lags; in lock step all receivers are equal) */
 int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *ctx, uint64_t *out, uint32_t n_rx);
+/* Restart receiver r of a ragged mixed-receivers context (VDL2GPU_FLAG_RAGGED) at the start of the next span that runs:
+ * from that span on, its channels decode exactly what a freshly started reference process tuned to (centerfreq, freqs)
+ * decodes from the samples the receiver brings from then on.  centerfreq 0 keeps the receiver's centre; freqs NULL keeps
+ * its channel frequencies, otherwise it holds rx[r].n_channels entries (the channel count, oversample and format stay).
+ * For a front-end whose receiver reconnects, re-enumerates with a gap in its stream, is swapped for another device, or is
+ * moved to other frequencies; every other receiver keeps its demodulator state and its bursts in flight.
+ *   - Any of the four span calls applies it; an all-zero ragged span is a no-op and leaves it pending.  Several receivers
+ *     may restart in the same span; restarting one twice before a span runs keeps the last tuning.  The receiver may
+ *     bring any count to that span, 0 included.
+ *   - Its position (vdl2gpu_get_receiver_positions), frames' sync_dec_index, trace dec_index and burst timestamps keep
+ *     counting in its own decimated samples; burst_seq keeps counting, so (channel, burst_seq, idx) never repeats, and the
+ *     per-channel counters are the sums over the old and the new process.
+ *   - The old process is treated as killed at the restart point: a burst already complete is delivered normally (with
+ *     the old frequency); a burst still in progress is dropped without a frame, a trace event or a counter change.
+ * Returns VDL2GPU_EINVAL, before the device is touched, for a NULL context, r >= n_rx, or any context but a ragged
+ * mixed-receivers one. */
+int vdl2gpu_restart_receiver(vdl2gpu_ctx *ctx, uint32_t r, uint32_t centerfreq, const uint32_t *freqs);
 int vdl2gpu_wait_input_consumed(vdl2gpu_ctx *ctx, void *stream);
 /* Make `stream` (cudaStream_t) wait for all device work enqueued by this context so far (for timing with
  * events recorded on the caller's stream, and for ordering consumers of device-side results). */
