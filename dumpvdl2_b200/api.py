@@ -64,6 +64,12 @@ class _Event(C.Structure):
                 ("i", C.c_int32 * 8), ("f", C.c_float * 8)]
 
 
+class _Burst(C.Structure):
+    _fields_ = [("channel", C.c_uint32), ("datalen_bits", C.c_uint32), ("nbits", C.c_uint32), ("syndrome", C.c_uint32),
+                ("frame_pwr", C.c_float), ("mag_nf", C.c_float), ("ppm_error", C.c_float), ("freq", C.c_uint32),
+                ("sync_dec_index", C.c_uint64), ("words", C.POINTER(C.c_uint32))]
+
+
 _FRAME_CB = C.CFUNCTYPE(None, C.POINTER(_Frame), C.c_void_p)
 _LIB = None
 
@@ -124,6 +130,8 @@ def load_library():
     L.vdl2gpu_launch_burst_fec.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
     L.vdl2gpu_parse_records.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, _FRAME_CB, C.c_void_p]
     L.vdl2gpu_stage_read_events.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.vdl2gpu_stage_queue_bursts.argtypes = [C.c_void_p, C.POINTER(_Burst), C.c_uint32]
+    L.vdl2gpu_stage_read_counters.argtypes = [C.c_void_p, C.c_void_p]
     _LIB = L
     return L
 

@@ -1677,6 +1677,63 @@ extern "C" int vdl2gpu_launch_burst_fec(vdl2gpu_stage *st, uint8_t *region, uint
 	return VDL2GPU_OK;
 }
 
+/* Queue n bursts exactly as K2 hands them over (vdl2_burst_complete): pop n slots from the device free list (burst i takes
+ * the i-th pop), write each slot's header and its first ceil(nbits / 32) words only - the slot's later words keep whatever
+ * an earlier burst left there - then ready[0..n), n_ready and free_top.  Synchronous. */
+static_assert(sizeof(vdl2gpu_burst) == 48, "vdl2gpu_burst is part of the ABI");
+extern "C" int vdl2gpu_stage_queue_bursts(vdl2gpu_stage *st, const vdl2gpu_burst *bursts, uint32_t n) {
+	if(!st || (n && !bursts)) return VDL2GPU_EINVAL;
+	for(uint32_t i = 0; i < n; i++) {
+		const vdl2gpu_burst &b = bursts[i];
+		if(b.channel >= st->n_ch || b.nbits > VDL2_MAX_BURST_BITS || (b.nbits && !b.words)) return VDL2GPU_EINVAL;
+	}
+	CU(cudaDeviceSynchronize());
+	vdl2_queue_ctl ctl;
+	CU(cudaMemcpy(&ctl, st->d_ctl, sizeof(ctl), cudaMemcpyDeviceToHost));
+	if(ctl.n_ready) return VDL2GPU_EINVAL;                   /* the previous queue has not been decoded yet */
+	if(ctl.free_top < 0 || n > (uint32_t)ctl.free_top) return VDL2GPU_ETOOBIG;
+	if(n == 0) return VDL2GPU_OK;
+	std::vector<int32_t> popped(n);
+	CU(cudaMemcpy(popped.data(), st->d_free + (ctl.free_top - (int32_t)n), (size_t)n * 4, cudaMemcpyDeviceToHost));
+	std::vector<uint32_t> ready(n);
+	std::vector<uint8_t> buf(sizeof(vdl2_burst_slot));
+	for(uint32_t i = 0; i < n; i++) {
+		const vdl2gpu_burst &b = bursts[i];
+		const int32_t slot = popped[n - 1u - i];                /* the free list is a stack: the top entry goes first */
+		vdl2_burst_slot *s = reinterpret_cast<vdl2_burst_slot *>(buf.data());
+		s->channel = b.channel; s->burst_seq = i; s->datalen_bits = b.datalen_bits; s->syndrome = b.syndrome; s->nbits = b.nbits;
+		s->frame_pwr = b.frame_pwr; s->mag_nf = b.mag_nf; s->ppm_error = b.ppm_error;
+		s->sync_lo = (uint32_t)b.sync_dec_index; s->sync_hi = (uint32_t)(b.sync_dec_index >> 32); s->freq = b.freq; s->pad = 0;
+		const size_t nw = (b.nbits + 31u) / 32u;
+		if(nw) memcpy(s->words, b.words, nw * 4);
+		CU(cudaMemcpy(&st->d_pool[slot], s, offsetof(vdl2_burst_slot, words) + nw * 4, cudaMemcpyHostToDevice));
+		ready[i] = (uint32_t)slot;
+	}
+	CU(cudaMemcpy(st->d_ready, ready.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
+	ctl.free_top -= (int32_t)n;
+	ctl.n_ready = n;
+	static_assert(offsetof(vdl2_queue_ctl, n_ready) == sizeof(int32_t), "free_top and n_ready are the first two fields");
+	CU(cudaMemcpy(st->d_ctl, &ctl, 2 * sizeof(uint32_t), cudaMemcpyHostToDevice));
+	return VDL2GPU_OK;
+}
+
+/* the stage's per-channel counters, 9 x uint64 per channel in the order of vdl2gpu_get_channel_counters.  Synchronises. */
+extern "C" int vdl2gpu_stage_read_counters(vdl2gpu_stage *st, uint64_t *out) {
+	if(!st || !out) return VDL2GPU_EINVAL;
+	CU(cudaDeviceSynchronize());
+	std::vector<uint32_t> k3((size_t)VDL2_NUM_COUNTERS * st->n_chp), sync(st->n_chp), hdr(st->n_chp);
+	CU(cudaMemcpy(k3.data(), st->d_counters, k3.size() * 4, cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy(sync.data(), st->d_k2 + (size_t)K2_CNT_SYNC * st->n_chp, st->n_chp * 4, cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy(hdr.data(), st->d_k2 + (size_t)K2_CNT_HDR_GOOD * st->n_chp, st->n_chp * 4, cudaMemcpyDeviceToHost));
+	for(uint32_t ch = 0; ch < st->n_ch; ch++) {              /* a stage maps channel c to slot c */
+		uint64_t *o = out + (size_t)ch * VDL2_NUM_COUNTERS;
+		for(int k = 0; k < VDL2_NUM_COUNTERS; k++) o[k] = k3[(size_t)k * st->n_chp + ch];
+		o[VDL2_CNT_SYNC_GOOD] = sync[ch];
+		o[VDL2_CNT_HDR_CRC_GOOD] = hdr[ch];
+	}
+	return VDL2GPU_OK;
+}
+
 extern "C" int vdl2gpu_stage_read_events(vdl2gpu_stage *st, vdl2gpu_event *out, uint32_t cap) {
 	if(!st || !out) return VDL2GPU_EINVAL;
 	if(!(st->cfg.flags & VDL2GPU_FLAG_TRACE)) return 0;

@@ -365,6 +365,28 @@ int vdl2gpu_parse_records(const uint8_t *region_host, uint32_t region_bytes, uin
 		vdl2gpu_frame_cb cb, void *user);
 /* trace events of the stage (VDL2GPU_FLAG_TRACE).  Synchronises the device. */
 int vdl2gpu_stage_read_events(vdl2gpu_stage *stage, vdl2gpu_event *out, uint32_t cap);
+/* Feeding K3 directly, for tests of the burst decoder that choose every burst themselves.
+ * vdl2gpu_stage_queue_bursts queues n bursts in the stage exactly as K2 hands them over, so that the next
+ * vdl2gpu_launch_burst_fec decodes them: it pops n burst-pool slots from the stage's device free list, writes each slot's
+ * metadata and only its first ceil(nbits / 32) words (later words keep what an earlier burst left in the slot, as after
+ * K2), and queues the slots in call order; burst i gets burst_seq = i.  Synchronous.  Returns VDL2GPU_EINVAL if bursts are
+ * already queued, a channel is out of range or nbits > 16843, and VDL2GPU_ETOOBIG if n exceeds the free slots (a stage has
+ * max(256, 3 x n_channels) slots; every launch of vdl2gpu_launch_burst_fec gives the slots it decoded back).
+ * vdl2gpu_stage_read_counters copies the per-channel counters, 9 x uint64 per channel in the order of
+ * vdl2gpu_get_channel_counters, to `out` (host, n_channels x 9).  Synchronises the device. */
+typedef struct {
+	uint32_t channel;            /* < n_channels */
+	uint32_t datalen_bits;       /* transmission length from the header (src/decode.c:222) */
+	uint32_t nbits;              /* bits in words[], the 25 header bits included */
+	uint32_t syndrome;           /* header syndrome */
+	float frame_pwr, mag_nf, ppm_error;
+	uint32_t freq;
+	uint64_t sync_dec_index;
+	const uint32_t *words;       /* HOST memory: the still-scrambled bits, bit i = words[i / 32] >> (31 - i % 32) & 1, the rest
+	                              * of the last word zero */
+} vdl2gpu_burst;                 /* 48 bytes */
+int vdl2gpu_stage_queue_bursts(vdl2gpu_stage *stage, const vdl2gpu_burst *bursts, uint32_t n);
+int vdl2gpu_stage_read_counters(vdl2gpu_stage *stage, uint64_t *out);
 
 #ifdef __cplusplus
 }

@@ -32,6 +32,7 @@ def test_abi_version_and_struct_sizes():
     assert L.vdl2gpu_abi_version() == 2
     from dumpvdl2_b200 import api
     assert C.sizeof(api._Config) == 72 and C.sizeof(api._Stats) == 160 and C.sizeof(api._Event) == 80
+    assert C.sizeof(api._Burst) == 48
 
 
 def test_no_cpu_fallback():

@@ -4,7 +4,7 @@ burst decoder.  This is how kernel logic is checked without a GPU; the -m gpu te
 import numpy as np
 import pytest
 from oracle import pyoracle as po
-from tests import cases, util
+from tests import cases, k3_corpus, util
 from tests.hostsim import pyhostsim as hs
 
 
@@ -192,122 +192,82 @@ def test_unwrap_transition_table_equals_the_double_arithmetic_of_the_reference()
             assert got.tobytes() == u.tobytes()
 
 
-def _flag():
-    return "01111110"
+def _check_k3(it):
+    """the host form of K3 on one corpus item equals the oracle's answer, FCS residues included"""
+    st, fr, corr, rs, crcs = hs.k3(it["bits"], it["datalen_bits"])
+    w = it["want"]
+    assert (st, fr, corr) == (w["status"], w["frames"], w["corr"]), (it["kind"], st, w["status"], len(fr), len(w["frames"]))
+    assert [int(r) for r in rs] == w["rs"], (it["kind"], list(rs), w["rs"])
+    assert [int(c) for c in crcs] == [po.crc16(f) for f in fr]
 
 
-def _stuffed(octets):
-    return "".join(format(b, "08b")[::-1] for b in octets).replace("11111", "111110")
+def _items(kind):
+    return [it for it in k3_corpus.corpus() if it["kind"] == kind]
 
 
 @pytest.mark.parametrize("trial", range(40))
 def test_burst_decoder_matches_oracle_on_hdlc_edge_cases(trial):
     """K3 device functions (de-interleave, RS, HDLC unstuff, FCS) against the oracle's restatement of
-    src/decode.c:259-380 + src/bitstream.c:109-150 on crafted payloads: repeated / missing flags, aborts (seven
-    ones), frames that are not whole octets, zero-length frames, length cuts, multi-block and short-block bursts,
-    RS errors within and beyond capacity."""
-    from dumpvdl2_b200 import synth
-    rng = np.random.default_rng(1000 + trial)
-    pieces = [_flag()]
-    for _ in range(int(rng.integers(1, 5))):
-        body = _stuffed(rng.integers(0, 256, int(rng.integers(0, 120)), dtype=np.uint8))
-        kind = int(rng.integers(0, 10))
-        if kind == 0:
-            body += "1" * 7                                   # abort sequence
-        elif kind == 1:
-            body += "010"                                     # not a whole number of octets
-        elif kind == 2:
-            body = ""                                         # back-to-back flags
-        pieces.append(body)
-        pieces.append(_flag() * int(rng.integers(1, 3)))
-    payload = "".join(pieces)
-    if trial % 5 == 0:
-        payload = payload[:-int(rng.integers(1, 8))]          # closing flag cut short
-    if trial % 7 == 0:
-        payload = _flag() + _stuffed(rng.integers(0, 256, int(rng.integers(250, 900)), dtype=np.uint8)) + _flag()
-    corrupt = []
-    nblk = -(-(-(-len(payload) // 8)) // 249)
-    for _ in range(int(rng.integers(0, 5))):
-        corrupt.append((int(rng.integers(0, nblk)), int(rng.integers(0, 20)), int(rng.integers(1, 256))))
-    try:
-        bits, info = synth.burst_bits_from_payload(payload, corrupt_octets=corrupt)
-    except ValueError:
+    src/decode.c:259-380 + src/bitstream.c:109-150 on crafted payloads (k3_corpus.hdlc_edge_payload): repeated / missing
+    flags, aborts (seven ones), frames that are not whole octets, back-to-back flags, length cuts, multi-block and
+    short-block bursts, RS errors within and beyond capacity."""
+    mine = [it for it in _items("hdlc_edge") if it["trial"] == trial]
+    if not mine:
         pytest.skip("payload too short for FEC")
-    descr = bits ^ synth.scrambler_sequence(len(bits))
-    st_o, fr_o, corr_o, rs_o = po.decode_burst_bits(descr[25:], info["datalen_bits"])
-    st_k, fr_k, corr_k, rs_k, crcs = hs.k3(bits, info["datalen_bits"])
-    assert (st_k, fr_k, corr_k) == (st_o, fr_o, corr_o), (st_k, st_o, len(fr_k), len(fr_o))
-    assert list(rs_k) == list(rs_o)
-    assert [int(c) for c in crcs] == [po.crc16(f) for f in fr_k]
+    _check_k3(mine[0])
 
 
-@pytest.mark.parametrize("n_octets", [1, 2, 3, 4, 30, 31, 32, 67, 68, 69, 248, 249, 250, 251, 252, 279, 280, 317, 498, 499, 747,
-                                      1245, 1992, 1993, 1994, 2022, 2023, 2040, 2046, 2047])
+@pytest.mark.parametrize("n_octets", k3_corpus.GEOMETRY_LENGTHS)
 def test_burst_decoder_block_geometry_edges(n_octets):
     """Block geometry corners of src/decode.c:124-133,222-297: last-block lengths around the FEC-octet thresholds
     (2|3, 30|31, 67|68), exact multiples of 249, and the maximum transmission length (9 blocks, 2047 octets),
     each with a couple of corrupted octets in the first and the last block."""
-    from dumpvdl2_b200 import synth
-    rng = np.random.default_rng(5000 + n_octets)
-    body = _flag() + _stuffed(rng.integers(0, 256, max(0, n_octets - 4), dtype=np.uint8)) + _flag()
-    payload = (body + _flag() * 300)[:n_octets * 8]           # pad with flags, cut to the exact transmission length
-    nblk = -(-n_octets // 249)
-    last_len = n_octets - (nblk - 1) * 249
-    corrupt = [(0, int(rng.integers(0, min(249, n_octets))), 0x55)]
-    if last_len > 2:
-        corrupt.append((nblk - 1, int(rng.integers(0, last_len)), 0xAA))
-    try:
-        bits, info = synth.burst_bits_from_payload(payload, corrupt_octets=corrupt)
-    except ValueError:
+    mine = [it for it in _items("geometry") if it["datalen_bits"] == 8 * n_octets]
+    if not mine:
         pytest.skip("no FEC octets for this length")
-    assert info["datalen_bits"] == n_octets * 8
-    descr = bits ^ synth.scrambler_sequence(len(bits))
-    st_o, fr_o, corr_o, rs_o = po.decode_burst_bits(descr[25:], info["datalen_bits"])
-    st_k, fr_k, corr_k, rs_k, crcs = hs.k3(bits, info["datalen_bits"])
-    assert (st_k, fr_k, corr_k) == (st_o, fr_o, corr_o), (st_k, st_o, len(fr_k), len(fr_o))
-    assert list(rs_k) == list(rs_o) and sum(int(r) != -128 for r in rs_k) == nblk
+    nblk = -(-n_octets // 249)
+    for it in mine:
+        _check_k3(it)
+        assert sum(r != -128 for r in it["want"]["rs"]) == nblk
 
 
 def test_burst_decoder_fuzz_random_payloads():
     """Random transmissions (any bit length 17..16383, random content with a sprinkling of flags, 0..8 corrupted octets
     anywhere in the code words): K3's device functions must return exactly the oracle's status, frames, correction
     count, per-block RS results and FCS residues."""
-    from dumpvdl2_b200 import synth
-    rng = np.random.default_rng(0xF0B8)
-    done = 0
-    for trial in range(240):
-        nbits = int(rng.integers(17, 0x4000)) if trial % 3 else int(rng.integers(17, 700))
-        if trial % 2:                                        # well-formed: stuffed frames between flags, cut to nbits
-            payload = _flag()
-            while len(payload) < nbits:
-                payload += _stuffed(rng.integers(0, 256, int(rng.integers(0, 300)), dtype=np.uint8)) + _flag() * int(rng.integers(1, 3))
-            if trial % 4 == 1:
-                payload = payload[:nbits]                    # cut anywhere
-            else:
-                nbits = len(payload) if len(payload) < 0x4000 else nbits
-                payload = payload[:nbits]
-        else:                                                # raw noise with a few flags dropped in
-            p_one = (0.5, 0.8, 0.65)[(trial // 2) % 3]          # ones-heavy noise: many stuffed zeros, flags and aborts
-            bits01 = (rng.random(nbits) < p_one).astype(np.uint8)
-            payload = "".join("01"[b] for b in bits01)
-            for _ in range(int(rng.integers(0, 6))):
-                at = int(rng.integers(0, max(1, nbits - 8)))
-                payload = payload[:at] + _flag() + payload[at + 8:]
-        n_oct = -(-nbits // 8)
-        nblk = -(-n_oct // 249)
-        corrupt = [(int(rng.integers(0, nblk)), int(rng.integers(0, 255)), int(rng.integers(1, 256)))
-                   for _ in range(int(rng.integers(0, 9)) if trial % 3 == 1 else 0)]
-        last_len = n_oct - (nblk - 1) * 249
-        corrupt = [(r, c, x) for (r, c, x) in corrupt if not (r == nblk - 1 and last_len <= c < 249)]   # keep to transmitted octets
-        try:
-            bits, info = synth.burst_bits_from_payload(payload, corrupt_octets=corrupt)
-        except ValueError:
+    mine = _items("fuzz")
+    for it in mine:
+        _check_k3(it)
+    assert len(mine) > 200
+
+
+def test_burst_corpus_matches_oracle_and_covers_every_rs_outcome():
+    """The rest of the burst corpus the GPU burst-decoder tests decode (tests/k3_corpus.py) through the host form of K3:
+    RS blocks past capacity, geometry lengths of 5-9 blocks, bursts of hundreds of frames, truncated bursts and the
+    one-block volume.  The corpus must hold every RS outcome, judged from the oracle's answers: correct decodes,
+    failures (deg(lambda) != number of roots), miscorrections, a failure in the first and in a middle block, a
+    miscorrected shortened last block; and more bursts than two grid-strides of K3."""
+    items = k3_corpus.corpus()
+    for it in items:
+        if it["kind"] not in ("hdlc_edge", "fuzz") and not (it["kind"] == "geometry" and it["datalen_bits"] // 8 in k3_corpus.GEOMETRY_LENGTHS):
+            _check_k3(it)
+    assert len(items) >= 2 * k3_corpus.K3_GRID
+    blocks = [b for it in items if it["kind"] == "rs" for b in it["blocks"]]
+    kinds = {k for k, _, _ in blocks}
+    assert {"ok", "fail", "miscorrect"} <= kinds
+    assert any(k == "miscorrect" and last and nfec == 2 for k, nfec, last in blocks)
+    assert any(k == "miscorrect" and last and nfec == 4 for k, nfec, last in blocks)
+    first = middle = 0
+    for it in items:
+        r, nblk = it["want"]["rs"], -(-it["datalen_bits"] // (8 * 249))
+        if it["kind"] != "rs" or nblk < 3 or -1 not in r:
             continue
-        descr = bits ^ synth.scrambler_sequence(len(bits))
-        st_o, fr_o, corr_o, rs_o = po.decode_burst_bits(descr[25:], info["datalen_bits"])
-        st_k, fr_k, corr_k, rs_k, crcs = hs.k3(bits, info["datalen_bits"])
-        assert (st_k, fr_k, corr_k) == (st_o, fr_o, corr_o), (trial, nbits, st_k, st_o, len(fr_k), len(fr_o))
-        assert list(rs_k) == list(rs_o), (trial, list(rs_k), list(rs_o))
-        assert [int(c) for c in crcs] == [po.crc16(f) for f in fr_k]
-        done += 1
-    assert done > 200
+        q = r.index(-1)
+        assert all(x == -128 for x in r[q + 1:])                # blocks after the failure are not run
+        first += q == 0
+        middle += 0 < q < nblk - 1
+    assert first and middle
+    status = {it["want"]["status"] for it in items}
+    assert {0, k3_corpus.ERR_FEC_BAD, k3_corpus.ERR_DATA_TRUNCATED, k3_corpus.ERR_FEC_TRUNCATED} <= status
+    assert max(len(it["want"]["frames"]) for it in items) > 128
+    assert any(it["datalen_bits"] == 8 * 2047 for it in items)
