@@ -123,7 +123,6 @@ struct vdl2gpu_ctx {
 	uint32_t k2a_split = 64;                            /* time slices of the K2a grid (VDL2GPU_K2A_SPLIT) */
 	int stages = 2;                                     /* 2: K2a runs alone between K1 of chunk c and K1 of chunk c+1 (default, see run_chain);
 	                                                     * 3: K2a of chunk c+1 beside K1 of chunk c+2 and K2 of chunk c (VDL2GPU_STAGES=3) */
-	bool fuse_phase = false;                            /* VDL2GPU_FUSE_PHASE=1: K1 writes the phase plane itself, no K2a launch (measured slower than the separate pass: DESIGN.md) */
 	bool k2a_exclusive = true;                          /* K1 of chunk c+1 waits for K2a of chunk c (VDL2GPU_K2A_EXCLUSIVE=0: let them overlap) */
 	uint64_t overflows_reported = 0;
 	host_tables tab;
@@ -283,14 +282,6 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 		if((e = getenv("VDL2GPU_K2A_EXCLUSIVE"))) c->k2a_exclusive = atoi(e) != 0;
 		if((e = getenv("VDL2GPU_STAGES")) && atoi(e) == 3) { c->stages = 3; c->k2a_split = 3; }
 		if((e = getenv("VDL2GPU_K2A_SPLIT")) && atoi(e) >= 1 && atoi(e) <= 256) c->k2a_split = (uint32_t)atoi(e);
-	}
-	{
-		/* fused phase pass (opt-in): needs the K1 kernel that implements it, the fast (Ziv-guarded) atan2 and a walk that takes its
-		 * magnitudes from the samples (no magnitude plane, hence nothing left for K2a to do) */
-		const char *e = getenv("VDL2GPU_FUSE_PHASE");
-		const int k2v = c->k2_variant & 0xFF;
-		c->fuse_phase = (e && atoi(e) != 0) && c->k2a_mode == 1 && !(k2v >= 0 && k2v <= 4) && c->stages == 2
-			&& vdl2_k1_fuses_phase(cfg->oversample, c->ch_per_stream, (cfg->flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->receivers ? 1 : 0);
 	}
 	if(cfg->flags & (VDL2GPU_FLAG_NO_GRAPH | VDL2GPU_FLAG_TRACE)) c->use_graphs = false;
 	c->freqs.assign(cfg->freqs, cfg->freqs + cfg->n_channels);
@@ -753,7 +744,6 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	p1.slot_rx = c->d_slot_rx; p1.block_rx = c->d_block_rx; p1.rx_tile = c->rx_tile; p1.rx_max = c->rx_max;
 	p1.rx_in = c->d_rx_in; p1.slot_cls = c->d_slot_cls; p1.cls_mask = c->cls_mask; p1.rx_os_max = c->rx_os_max;
 	memcpy(p1.cls_taps, c->cls_taps, sizeof(p1.cls_taps));
-	p1.phase = c->fuse_phase ? c->d_phase2[pb] : nullptr; p1.phase_prev = c->d_phase2[pb ^ 1]; p1.prev_n_dec = prev_n_dec;
 	/* the default walk (variant 5) computes the four magnitudes a block needs from the staged samples: no magnitude plane */
 	const bool need_mag = (c->k2_variant & 0xFF) >= 0 && (c->k2_variant & 0xFF) <= 4;
 	pa.dec = d_dec; pa.phase = c->d_phase2[pb]; pa.mag = need_mag ? c->d_mag2[pb] : nullptr; pa.phase_prev = c->d_phase2[pb ^ 1];
@@ -853,7 +843,7 @@ static int ensure_graphs(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n
 	if(s.g_back[k]) { cudaGraphExecDestroy(s.g_back[k]); s.g_back[k] = nullptr; }
 	capture_env e = { c, &s, seq, n_pairs, k0_fmt };
 	int rc = capture_one(c->stream, &s.g_front[k], body_front, &e);
-	if(rc == 0 && !c->fuse_phase) rc = capture_one(c->s_mid, &s.g_k2a[k], body_k2a, &e);
+	if(rc == 0) rc = capture_one(c->s_mid, &s.g_k2a[k], body_k2a, &e);
 	if(rc == 0) rc = capture_one(c->s_back, &s.g_back[k], body_back, &e);
 	if(rc == 0) s.graph_pairs[k] = n_pairs;
 	return rc;
@@ -887,16 +877,12 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 		s.h_args->n_dec = s.n_dec; s.h_args->prev_n_dec = c->last_n_dec;
 	}
 	/* ---- front stage: K0, K1 -> dec[db] (free once K2 of chunk c-3 is done) ---- */
-	/* Fused phase pass: K1 also writes phase plane pb, which the walk of chunk c-2 read; the front stage then runs in lock
-	 * step with the back stage of chunk c-1 - K1(c) and K2(c-1) start together once K3(c-2) has finished, again one block per
-	 * SM each into an empty machine - and there is no middle stage. */
-	if(c->fuse_phase) { if(seq >= 2 && overlap) CU(cudaStreamWaitEvent(c->stream, c->ev_back_done[(seq - 2) % 3u], 0)); }
-	else if(seq >= 3) CU(cudaStreamWaitEvent(c->stream, c->ev_back_done[db], 0));
+	if(seq >= 3) CU(cudaStreamWaitEvent(c->stream, c->ev_back_done[db], 0));
 	/* Two-stage schedule (default): K1 of this chunk starts when K2a of the previous chunk has finished.  K2a is a short
 	 * full-occupancy pass; when it ends the GPU is empty, and K2 of chunk c-1 and K1 of chunk c are then launched into that
 	 * empty machine together, one block per SM each - the only arrangement in which the block scheduler was found to keep
 	 * the two long kernels side by side on every SM, launch after launch (see the slot mapping in create_impl). */
-	if(!c->fuse_phase && c->stages == 2 && seq >= 1 && overlap) CU(cudaStreamWaitEvent(c->stream, c->ev_k2a_done[pb ^ 1], 0));
+	if(c->stages == 2 && seq >= 1 && overlap) CU(cudaStreamWaitEvent(c->stream, c->ev_k2a_done[pb ^ 1], 0));
 	if(s.timed) { CU(cudaEventRecord(s.tk[0], c->stream)); if(graph) CU(cudaEventRecord(s.tk[1], c->stream)); }
 	if(graph) {
 		CU(cudaGraphLaunch(s.g_front[gk], c->stream));
@@ -915,25 +901,20 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	CU(cudaEventRecord(c->ev_input_consumed, c->stream));
 	CU(cudaEventRecord(c->ev_k1_done[db], c->stream));
 	/* ---- middle stage: K2a -> plane[pb] (free once K2 of chunk c-2 is done), history from plane[pb ^ 1] (chunk c-1, same stream) ---- */
-	if(c->fuse_phase) {
-		if(s.timed) { CU(cudaEventRecord(s.tk[3], c->stream)); CU(cudaEventRecord(s.tk[6], c->stream)); }
-		CU(cudaEventRecord(c->ev_k2a_done[pb], c->stream));
-	} else {
-		CU(cudaStreamWaitEvent(c->s_mid, c->ev_k1_done[db], 0));
-		if(seq >= 2 && overlap) CU(cudaStreamWaitEvent(c->s_mid, c->ev_back_done[(seq - 2) % 3u], 0));
-		if(s.timed) CU(cudaEventRecord(s.tk[3], c->s_mid));
-		if(graph) CU(cudaGraphLaunch(s.g_k2a[gk], c->s_mid));
-		else KL(vdl2_launch_k2a_warps(&pa, c->s_mid));
-		if(s.timed) CU(cudaEventRecord(s.tk[6], c->s_mid));
-		CU(cudaEventRecord(c->ev_k2a_done[pb], c->s_mid));
-	}
+	CU(cudaStreamWaitEvent(c->s_mid, c->ev_k1_done[db], 0));
+	if(seq >= 2 && overlap) CU(cudaStreamWaitEvent(c->s_mid, c->ev_back_done[(seq - 2) % 3u], 0));
+	if(s.timed) CU(cudaEventRecord(s.tk[3], c->s_mid));
+	if(graph) CU(cudaGraphLaunch(s.g_k2a[gk], c->s_mid));
+	else KL(vdl2_launch_k2a_warps(&pa, c->s_mid));
+	if(s.timed) CU(cudaEventRecord(s.tk[6], c->s_mid));
+	CU(cudaEventRecord(c->ev_k2a_done[pb], c->s_mid));
 	/* ---- back stage: K2, K3 ---- */
 	CU(cudaStreamWaitEvent(c->s_back, c->ev_k2a_done[pb], 0));
 	if(s.timed) CU(cudaEventRecord(s.tk[7], c->s_back));
 	if(graph) {
 		CU(cudaGraphLaunch(s.g_back[gk], c->s_back));
 		if(s.timed) CU(cudaEventRecord(s.tk[4], c->s_back));
-		c->stats.graph_launches += c->fuse_phase ? 2 : 3;
+		c->stats.graph_launches += 3;
 	} else {
 		KL(vdl2_launch_k2(&p2, c->s_back));
 		if(s.timed) CU(cudaEventRecord(s.tk[4], c->s_back));
@@ -954,7 +935,7 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	if(c->ragged) for(uint32_t r = 0; r < c->n_streams; r++) c->stats.iq_samples += (uint64_t)s.h_span[r].n * c->rx_in[r].oversample;
 	else c->stats.iq_samples += c->mixed ? (uint64_t)n_pairs * c->span_pairs_per_dec : n_pairs;
 	c->stats.dec_samples += s.n_dec;
-	c->stats.kernel_launches += (n_pairs ? 2 : 0) + (c->fuse_phase ? 0 : 1) + (s.n_dec ? 1 : 0) + 2;
+	c->stats.kernel_launches += (n_pairs ? 2 : 0) + 1 + (s.n_dec ? 1 : 0) + 2;
 	return VDL2GPU_OK;
 }
 

@@ -283,8 +283,11 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
 	asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count));
 }
 __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tma_load_tile(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+/* arm the barrier for `bytes` more bytes (one arrival), then issue copies that complete that many bytes on it */
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
 	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void tma_copy(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
 	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
 			:: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
@@ -317,24 +320,98 @@ __device__ __forceinline__ float4 k1_lut_entry(const float4 *s_lut, uint32_t pha
 /* break-point table of vdl2_phase_fast: constant memory, copied to shared memory by the kernels that use it */
 __constant__ double c_atan_tab[VDL2_ATAN_TABLE_DOUBLES] = VDL2_ATAN_TABLE_INIT;
 
-/* PH (fused phase pass, opt-in: VDL2GPU_FUSE_PHASE=1): the thread also produces the phase of every decimated sample it
- * writes.  In the tile loop the atan2 of group g-1's output is written out as straight-line code at the top of group g's
- * unrolled body (vdl2_phase_fast_nb: ~20 FP64 operations and their conversions, no branch) so that it can be scheduled
- * into the group's FP32 filter recurrence; the Ziv fall-back (about one sample in a million) and the store come at the
- * end of the body.  Measured: 6.4 instead of 5.0 ms per launch, more than the separate K2a pass costs (DESIGN.md section 4). */
-__device__ __forceinline__ float k1_phase_exact(float re, float im, const double *tab) {
-	int slow;
-	float f = vdl2_phase_fast_nb(re, im, tab, &slow);
-	if(slow) f = vdl2_phase_of(re, im);
-	return f;
+/* the packed constants of a filter with taps {a0, a1, a2} / {1, b1, b2} */
+__device__ __forceinline__ k1_packed_consts k1_consts(const vdl2_k1_params &p, float a0, float a1, float a2, float b1, float b2) {
+	k1_packed_consts c;
+	c.ONE = f2_pack(p.one, p.one); c.SGN = f2_pack(p.neg_one, p.one);
+	c.A0 = f2_pack(a0, a0); c.A1 = f2_pack(a1, a1); c.A2 = f2_pack(a2, a2);
+	c.B1 = f2_pack(b1, b1); c.B2 = f2_pack(b2, b2); c.TWO = f2_pack(p.two, p.two);
+	c.one = p.one; c.neg_one = p.neg_one;
+	return c;
 }
 
-template<int OS, int BLOCK, int BATCH, bool SYM, bool PH = false>
+/* k1_load_state / k1_store_state with the delay lines as (I, Q) pairs; without `load` the delay lines are zero and phi,
+ * dphi keep their values */
+__device__ __forceinline__ void k1_load_packed(const vdl2_k1_params &p, uint32_t ch, bool load, u64 &x1, u64 &x2, u64 &y1, u64 &y2,
+		uint32_t &phi, uint32_t &dphi) {
+	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
+	if(load) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
+	x1 = f2_pack(xr1, xi1); x2 = f2_pack(xr2, xi2); y1 = f2_pack(yr1, yi1); y2 = f2_pack(yr2, yi2);
+}
+__device__ __forceinline__ void k1_store_packed(const vdl2_k1_params &p, uint32_t ch, u64 x1, u64 x2, u64 y1, u64 y2, uint32_t phi) {
+	k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+}
+
+/* Samples [pos, end) one at a time through k1_packed_step, sample i at samples[i * stride + col]; every OS-th output (counted by
+ * cnt) is decimated sample m.  The head (samples up to the first decimation-group boundary) and the tail (fewer than OS
+ * samples after the last whole group) of the kernels that stage whole groups, read straight from global memory. */
+template<int OS, int NLUT>
+__device__ __forceinline__ void k1_sample_loop(const vdl2_k1_params &p, uint32_t ch, const float2 *samples, size_t stride, uint32_t col,
+		uint32_t &pos, uint32_t end, uint32_t &cnt, uint32_t &m, const float4 *lut, uint32_t &phi, const uint32_t dphi,
+		u64 &x1, u64 &x2, u64 &y1, u64 &y2, const k1_packed_consts &c) {
+	for(; pos < end; pos++) {
+		u64 y0 = k1_packed_step(samples[(size_t)pos * stride + col], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
+		if(++cnt == OS) { cnt = 0; p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0)); m++; }
+	}
+}
+
+/* One decimation group: OS samples, sample k at sp[k * SS], through NCO, mixer and filter; returns the group's last
+ * output, the decimated sample.  The K1 kernels that stage samples in shared memory run their groups through this body
+ * (the receiver-group kernel restates it, see there).
+ * It is k1_packed_step's arithmetic operation for operation (no contraction, the same rounding order), written out as a
+ * software pipeline over the unrolled group: the loads run LA samples ahead of the mixer, the mixer MA samples ahead of
+ * the filter recurrence.
+ * SYM: the feed-forward taps of this filter design are {A0, 2*A0, A0} (checked on the host).  A1*x[n-1] and A2*x[n-2]
+ * are then exactly 2*(A0*x[n-1]) and A0*x[n-2], products the previous two steps already formed (doubling is exact; no
+ * operand can be subnormal here, see DESIGN.md), so two multiplies per sample go away: t = fma(P1, 2, P2) rounds once,
+ * exactly like A1*x1 + A2*x2.  P1 = A0*x1 and P2 = A0*x2 on entry and on return. */
+template<int OS, int NLUT, int SS, bool SYM>
+__device__ __forceinline__ u64 k1_group(const float2 *sp, const float4 *s_lut, uint32_t lane_bytes, uint32_t &phi, const uint32_t dphi,
+		u64 &x1, u64 &x2, u64 &y1, u64 &y2, u64 &P1, u64 &P2, const k1_packed_consts &c) {
+	constexpr int LA = 10, MA = 5;
+	u64 y0 = 0;
+	float2 S[OS];
+	float4 E[OS];
+	float FR[OS];
+	u64 X0[OS];
+#pragma unroll
+	for(int k = -LA; k < OS; k++) {
+		const int kl = k + LA, km = k + MA;
+		if(kl < OS) {
+			const uint32_t ph = phi + (uint32_t)kl * dphi;
+			E[kl] = k1_lut_entry<NLUT>(s_lut, ph, lane_bytes);
+			FR[kl] = (float)(ph & 0xFFFFu);
+			S[kl] = sp[kl * SS];
+		}
+		if(km >= 0 && km < OS) {
+			const u64 CS = f2_fma(f2_mul(f2_pack(E[km].z, E[km].w), f2_pack(FR[km], FR[km])), c.ONE, f2_pack(E[km].x, E[km].y));
+			X0[km] = k1_mix(S[km], CS, c);
+		}
+		if(k >= 0) {
+			const u64 x0 = X0[k];
+			u64 r;
+			if(SYM) {
+				const u64 P0 = f2_mul(c.A0, x0);
+				r = f2_fma(P0, c.ONE, f2_fma(P1, c.TWO, P2));
+				P2 = P1; P1 = P0;
+			} else {
+				const u64 t = f2_fma(f2_mul(c.A1, x1), c.ONE, f2_mul(c.A2, x2));
+				r = f2_fma(f2_mul(c.A0, x0), c.ONE, t);
+			}
+			const u64 u = f2_fma(f2_mul(c.B1, y1), c.ONE, f2_mul(c.B2, y2));
+			y0 = f2_fma(r, c.ONE, u);
+			x2 = x1; x1 = x0; y2 = y1; y1 = y0;
+		}
+	}
+	phi += (uint32_t)OS * dphi;
+	return y0;
+}
+
+/* BATCH = 0: the group as OS plain k1_packed_step calls (the un-pipelined A/B variant, VDL2GPU_K1_VARIANT=0), else k1_group */
+template<int OS, int BLOCK, int BATCH, bool SYM>
 __global__ void __launch_bounds__(BLOCK) k1_mix_iir_decimate_packed(vdl2_k1_params p) {
 	constexpr int TG = K1P_TILE_GROUPS(OS);
 	constexpr int NLUT = BLOCK >= 128 ? 8 : 1;                    /* table copies */
-	static_assert(!PH || (BATCH != 0 && BLOCK >= VDL2_ATAN_TABLE_DOUBLES), "fused phase pass: pipelined kernel only");
-	__shared__ double s_atan[PH ? VDL2_ATAN_TABLE_DOUBLES : 1];
 	__shared__ float4 s_lut[257 * NLUT];
 	__shared__ __align__(128) float2 s_tiles[2][TG * OS + 2];
 	__shared__ __align__(8) uint64_t s_bar[2];
@@ -349,52 +426,21 @@ __global__ void __launch_bounds__(BLOCK) k1_mix_iir_decimate_packed(vdl2_k1_para
 	const float4 *lut = s_lut + (NLUT > 1 ? (tid & (NLUT - 1)) : 0);       /* this lane's copy; entry i at lut[i * NLUT] */
 	const uint32_t lane_bytes = NLUT > 1 ? (tid & (NLUT - 1)) * 16u : 0u;
 	if(tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
-	if(PH && tid < VDL2_ATAN_TABLE_DOUBLES) s_atan[tid] = c_atan_tab[tid];
-	float *phase = nullptr;                                   /* this slot's column, row 0 = first sample of the chunk */
-	if(PH && active) {
-		/* history prefix: the last 160 phase rows of the previous chunk (src/demod.c:105-198 looks 150 samples back) */
-		const uint32_t prev_n_dec = p.ca ? p.ca->prev_n_dec : p.prev_n_dec;
-		const float *src = p.phase_prev + (size_t)prev_n_dec * p.n_chp + ch;
-		float *dst = p.phase + ch;
-#pragma unroll 8
-		for(uint32_t i = 0; i < VDL2_SYNC_BUFLEN; i++) dst[(size_t)i * p.n_chp] = src[(size_t)i * p.n_chp];
-		phase = p.phase + (size_t)VDL2_SYNC_BUFLEN * p.n_chp + ch;
-	}
-	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
+	u64 x1, x2, y1, y2;
 	uint32_t phi = 0, dphi = 0;
-	if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
-	u64 x1 = f2_pack(xr1, xi1), x2 = f2_pack(xr2, xi2), y1 = f2_pack(yr1, yi1), y2 = f2_pack(yr2, yi2);
-	k1_packed_consts c;
-	c.ONE = f2_pack(p.one, p.one); c.SGN = f2_pack(p.neg_one, p.one);
-	c.A0 = f2_pack(p.a0, p.a0); c.A1 = f2_pack(p.a1, p.a1); c.A2 = f2_pack(p.a2, p.a2);
-	c.B1 = f2_pack(p.b1, p.b1); c.B2 = f2_pack(p.b2, p.b2); c.TWO = f2_pack(p.two, p.two);
-	c.one = p.one; c.neg_one = p.neg_one;
-	/* SYM: the feed-forward taps of this filter design are {A0, 2*A0, A0} (checked on the host).  A1*x[n-1] and
-	 * A2*x[n-2] are then exactly 2*(A0*x[n-1]) and A0*x[n-2], products the previous two steps already formed
-	 * (doubling is exact; no operand can be subnormal here, see DESIGN.md), so two multiplies per sample go away:
-	 * t = fma(P1, 2, P2) rounds once, exactly like A1*x1 + A2*x2. */
-	u64 P1 = f2_mul(c.A0, x1), P2 = f2_mul(c.A0, x2);
+	k1_load_packed(p, ch, active, x1, x2, y1, y2, phi, dphi);
+	const k1_packed_consts c = k1_consts(p, p.a0, p.a1, p.a2, p.b1, p.b2);
 	__syncthreads();
 
 	uint32_t cnt = cnt0, m = 0, pos = 0;
 	/* head: samples up to the first decimation-group boundary, straight from global memory */
 	const uint32_t head = min(n_pairs, (OS - cnt0 % OS) % OS);
-	if(active) {
-		for(; pos < head; pos++) {
-			u64 y0 = k1_packed_step(samples[pos], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
-			if(++cnt == OS) {
-				cnt = 0;
-				p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0));
-				if(PH) phase[(size_t)m * p.n_chp] = k1_phase_exact(f2_lo(y0), f2_hi(y0), s_atan);
-				m++;
-			}
-		}
-	}
+	if(active) k1_sample_loop<OS, NLUT>(p, ch, samples, 1, 0, pos, head, cnt, m, lut, phi, dphi, x1, x2, y1, y2, c);
 	/* same bookkeeping for every lane, active or not */
 	pos = head;
 	m = (cnt0 + head) / OS;
 	cnt = (cnt0 + head) % OS;
-	P1 = f2_mul(c.A0, x1); P2 = f2_mul(c.A0, x2);            /* after the head samples */
+	u64 P1 = f2_mul(c.A0, x1), P2 = f2_mul(c.A0, x2);            /* after the head samples */
 	/* body: whole groups, staged through shared memory tile by tile */
 	const uint32_t n_groups = (n_pairs - pos) / OS;
 	const uint32_t n_tiles = (n_groups + TG - 1) / TG;
@@ -406,7 +452,9 @@ __global__ void __launch_bounds__(BLOCK) k1_mix_iir_decimate_packed(vdl2_k1_para
 	auto request_tile = [&](uint32_t t, uint32_t buf) {              /* thread 0 only */
 		const uint32_t n = min((uint32_t)TG, n_groups - t * TG) * OS + mis;
 		const float2 *src = samples + head + (size_t)t * TG * OS - mis;
-		tma_load_tile(s_tiles[buf], src, (n & ~1u) * (uint32_t)sizeof(float2), &s_bar[buf]);
+		const uint32_t bytes = (n & ~1u) * (uint32_t)sizeof(float2);
+		mbar_expect_tx(&s_bar[buf], bytes);
+		tma_copy(s_tiles[buf], src, bytes, &s_bar[buf]);
 		if(n & 1u) s_tiles[buf][n - 1] = src[n - 1];
 	};
 	if(tid == 0)
@@ -414,8 +462,6 @@ __global__ void __launch_bounds__(BLOCK) k1_mix_iir_decimate_packed(vdl2_k1_para
 	__syncthreads();
 	/* the tile loop, compiled twice: with the tile known to start on element 0 the compiler fetches two samples per
 	 * LDS.128; the misaligned case (odd decimation phase on entry) reads from element 1 with 64-bit loads */
-	u64 yprev = f2_pack(1.0f, 0.0f);                              /* output of the previous group, its phase still owed */
-	bool owed = false;
 	auto tile_loop = [&](auto MIS) {
 	for(uint32_t g0 = 0, tile = 0; g0 < n_groups; g0 += TG, tile++) {
 		const uint32_t ng = min((uint32_t)TG, n_groups - g0);
@@ -425,61 +471,12 @@ __global__ void __launch_bounds__(BLOCK) k1_mix_iir_decimate_packed(vdl2_k1_para
 			for(uint32_t g = 0; g < ng; g++) {
 				const float2 *sp = &s_tile[g * OS];
 				u64 y0 = 0;
-				float ph_prev = 0.0f;
-				int ph_slow = 0;
-				if(PH) ph_prev = vdl2_phase_fast_nb(f2_lo(yprev), f2_hi(yprev), s_atan, &ph_slow);
 				if(BATCH == 0) {
 #pragma unroll
 					for(int k = 0; k < OS; k++)
 						y0 = k1_packed_step(sp[k], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
-				} else {
-					/* software pipeline written out over the unrolled group: loads run LA samples ahead of the
-					 * mixer, the mixer MA samples ahead of the filter recurrence */
-					constexpr int LA = BATCH, MA = BATCH / 2;
-					float2 S[OS];
-					float4 E[OS];
-					float FR[OS];
-					u64 X0[OS];
-#pragma unroll
-					for(int k = -LA; k < OS; k++) {
-						const int kl = k + LA, km = k + MA;
-						if(kl < OS) {
-							const uint32_t ph = phi + (uint32_t)kl * dphi;
-							E[kl] = k1_lut_entry<NLUT>(s_lut, ph, lane_bytes);
-							FR[kl] = (float)(ph & 0xFFFFu);
-							S[kl] = sp[kl];
-						}
-						if(km >= 0 && km < OS) {
-							const u64 CS = f2_fma(f2_mul(f2_pack(E[km].z, E[km].w), f2_pack(FR[km], FR[km])), c.ONE, f2_pack(E[km].x, E[km].y));
-							X0[km] = k1_mix(S[km], CS, c);
-						}
-						if(k >= 0) {
-							const u64 x0 = X0[k];
-							u64 r;
-							if(SYM) {
-								const u64 P0 = f2_mul(c.A0, x0);
-								r = f2_fma(P0, c.ONE, f2_fma(P1, c.TWO, P2));
-								P2 = P1; P1 = P0;
-							} else {
-								const u64 t = f2_fma(f2_mul(c.A1, x1), c.ONE, f2_mul(c.A2, x2));
-								r = f2_fma(f2_mul(c.A0, x0), c.ONE, t);
-							}
-							const u64 u = f2_fma(f2_mul(c.B1, y1), c.ONE, f2_mul(c.B2, y2));
-							y0 = f2_fma(r, c.ONE, u);
-							x2 = x1; x1 = x0; y2 = y1; y1 = y0;
-						}
-					}
-					phi += (uint32_t)OS * dphi;
-				}
+				} else y0 = k1_group<OS, NLUT, 1, SYM>(sp, s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
 				p.dec[(size_t)(m + g) * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0));
-				if(PH) {
-					if(owed) {
-						if(ph_slow) ph_prev = vdl2_phase_of(f2_lo(yprev), f2_hi(yprev));
-						phase[(size_t)(m + g - 1u) * p.n_chp] = ph_prev;
-					}
-					yprev = y0;
-					owed = true;
-				}
 			}
 		}
 		m += ng;
@@ -489,19 +486,10 @@ __global__ void __launch_bounds__(BLOCK) k1_mix_iir_decimate_packed(vdl2_k1_para
 	}
 	};
 	if(mis) tile_loop(std::integral_constant<int, 1>{}); else tile_loop(std::integral_constant<int, 0>{});
-	if(PH && active && owed) phase[(size_t)(m - 1u) * p.n_chp] = k1_phase_exact(f2_lo(yprev), f2_hi(yprev), s_atan);
 	/* tail: fewer than OS samples left */
 	if(active) {
-		for(; pos < n_pairs; pos++) {
-			u64 y0 = k1_packed_step(samples[pos], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
-			if(++cnt == OS) {
-				cnt = 0;
-				p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0));
-				if(PH) phase[(size_t)m * p.n_chp] = k1_phase_exact(f2_lo(y0), f2_hi(y0), s_atan);
-				m++;
-			}
-		}
-		k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+		k1_sample_loop<OS, NLUT>(p, ch, samples, 1, 0, pos, n_pairs, cnt, m, lut, phi, dphi, x1, x2, y1, y2, c);
+		k1_store_packed(p, ch, x1, x2, y1, y2, phi);
 	}
 	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);
 }
@@ -521,7 +509,6 @@ __global__ void __launch_bounds__(BLOCK) k1_mix_iir_decimate_packed(vdl2_k1_para
 template<int OS, bool SYM>
 __global__ void __launch_bounds__(K1L_BLOCK) k1_mix_iir_decimate_lanes(vdl2_k1_params p) {
 	constexpr int TG = K1L_TILE_ROWS / OS;                 /* groups per tile */
-	constexpr int LA = 10, MA = 5;
 	constexpr int NLUT = 8;
 	extern __shared__ __align__(128) unsigned char k1l_smem[];
 	float2 *s_tiles = reinterpret_cast<float2 *>(k1l_smem);                                            /* [2][TG*OS][128] */
@@ -538,27 +525,17 @@ __global__ void __launch_bounds__(K1L_BLOCK) k1_mix_iir_decimate_lanes(vdl2_k1_p
 	const float4 *lut = s_lut + (tid & (NLUT - 1));
 	const uint32_t lane_bytes = (tid & (NLUT - 1)) * 16u;
 	if(tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
-	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
+	u64 x1, x2, y1, y2;
 	uint32_t phi = 0, dphi = 0;
-	if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
-	u64 x1 = f2_pack(xr1, xi1), x2 = f2_pack(xr2, xi2), y1 = f2_pack(yr1, yi1), y2 = f2_pack(yr2, yi2);
-	k1_packed_consts c;
-	c.ONE = f2_pack(p.one, p.one); c.SGN = f2_pack(p.neg_one, p.one);
-	c.A0 = f2_pack(p.a0, p.a0); c.A1 = f2_pack(p.a1, p.a1); c.A2 = f2_pack(p.a2, p.a2);
-	c.B1 = f2_pack(p.b1, p.b1); c.B2 = f2_pack(p.b2, p.b2); c.TWO = f2_pack(p.two, p.two);
-	c.one = p.one; c.neg_one = p.neg_one;
+	k1_load_packed(p, ch, active, x1, x2, y1, y2, phi, dphi);
+	const k1_packed_consts c = k1_consts(p, p.a0, p.a1, p.a2, p.b1, p.b2);
 	/* the last block may reach past the allocated columns when n_chp is not a multiple of 128: clamp the column */
 	const uint32_t col = min(tid, (uint32_t)(p.stream_stride - 1 - (size_t)blockIdx.x * K1L_BLOCK));
 	__syncthreads();
 
 	uint32_t cnt = cnt0, m = 0, pos = 0;
 	const uint32_t head = min(n_pairs, (OS - cnt0 % OS) % OS);
-	if(active) {
-		for(; pos < head; pos++) {
-			u64 y0 = k1_packed_step(samples[(size_t)pos * stride + col], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
-			if(++cnt == OS) { cnt = 0; p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0)); m++; }
-		}
-	}
+	if(active) k1_sample_loop<OS, NLUT>(p, ch, samples, stride, col, pos, head, cnt, m, lut, phi, dphi, x1, x2, y1, y2, c);
 	pos = head;
 	m = (cnt0 + head) / OS;
 	cnt = (cnt0 + head) % OS;
@@ -571,15 +548,13 @@ __global__ void __launch_bounds__(K1L_BLOCK) k1_mix_iir_decimate_lanes(vdl2_k1_p
 	 * one row each (`request`, after it) */
 	auto arm = [&](uint32_t t, uint32_t buf) {
 		const uint32_t rows = min((uint32_t)TG, n_groups - t * TG) * OS;
-		if(tid == 0)
-			asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(&s_bar[buf])), "r"(rows * row_bytes) : "memory");
+		if(tid == 0) mbar_expect_tx(&s_bar[buf], rows * row_bytes);
 	};
 	auto request = [&](uint32_t t, uint32_t buf) {
 		const uint32_t rows = min((uint32_t)TG, n_groups - t * TG) * OS;
 		const float2 *src = samples + (size_t)(head + (size_t)t * TG * OS) * stride;
 		for(uint32_t r = tid; r < rows; r += K1L_BLOCK)
-			asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-					:: "r"(smem_u32(&s_tiles[((size_t)buf * TG * OS + r) * K1L_BLOCK])), "l"(src + (size_t)r * stride), "r"(row_bytes), "r"(smem_u32(&s_bar[buf])) : "memory");
+			tma_copy(&s_tiles[((size_t)buf * TG * OS + r) * K1L_BLOCK], src + (size_t)r * stride, row_bytes, &s_bar[buf]);
 	};
 	for(uint32_t t = 0; t < 2 && t < n_tiles; t++) arm(t, t);
 	__syncthreads();
@@ -590,42 +565,8 @@ __global__ void __launch_bounds__(K1L_BLOCK) k1_mix_iir_decimate_lanes(vdl2_k1_p
 		mbar_wait(&s_bar[tile & 1u], (tile >> 1) & 1u);
 		if(active) {
 			for(uint32_t g = 0; g < ng; g++) {
-				const float2 *sp = &s_tile[g * OS * K1L_BLOCK];
-				u64 y0 = 0;
-				float2 S[OS];
-				float4 E[OS];
-				float FR[OS];
-				u64 X0[OS];
-#pragma unroll
-				for(int k = -LA; k < OS; k++) {
-					const int kl = k + LA, km = k + MA;
-					if(kl < OS) {
-						const uint32_t ph = phi + (uint32_t)kl * dphi;
-						E[kl] = k1_lut_entry<NLUT>(s_lut, ph, lane_bytes);
-						FR[kl] = (float)(ph & 0xFFFFu);
-						S[kl] = sp[kl * K1L_BLOCK];
-					}
-					if(km >= 0 && km < OS) {
-						const u64 CS = f2_fma(f2_mul(f2_pack(E[km].z, E[km].w), f2_pack(FR[km], FR[km])), c.ONE, f2_pack(E[km].x, E[km].y));
-						X0[km] = k1_mix(S[km], CS, c);
-					}
-					if(k >= 0) {
-						const u64 x0 = X0[k];
-						u64 r;
-						if(SYM) {
-							const u64 P0 = f2_mul(c.A0, x0);
-							r = f2_fma(P0, c.ONE, f2_fma(P1, c.TWO, P2));
-							P2 = P1; P1 = P0;
-						} else {
-							const u64 t = f2_fma(f2_mul(c.A1, x1), c.ONE, f2_mul(c.A2, x2));
-							r = f2_fma(f2_mul(c.A0, x0), c.ONE, t);
-						}
-						const u64 u = f2_fma(f2_mul(c.B1, y1), c.ONE, f2_mul(c.B2, y2));
-						y0 = f2_fma(r, c.ONE, u);
-						x2 = x1; x1 = x0; y2 = y1; y1 = y0;
-					}
-				}
-				phi += (uint32_t)OS * dphi;
+				const u64 y0 = k1_group<OS, NLUT, K1L_BLOCK, SYM>(&s_tile[g * OS * K1L_BLOCK], s_lut, lane_bytes, phi, dphi,
+						x1, x2, y1, y2, P1, P2, c);
 				p.dec[(size_t)(m + g) * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0));
 			}
 		}
@@ -636,11 +577,8 @@ __global__ void __launch_bounds__(K1L_BLOCK) k1_mix_iir_decimate_lanes(vdl2_k1_p
 		if(tile + 2 < n_tiles) request(tile + 2, tile & 1u);
 	}
 	if(active) {
-		for(; pos < n_pairs; pos++) {
-			u64 y0 = k1_packed_step(samples[(size_t)pos * stride + col], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
-			if(++cnt == OS) { cnt = 0; p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0)); m++; }
-		}
-		k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+		k1_sample_loop<OS, NLUT>(p, ch, samples, stride, col, pos, n_pairs, cnt, m, lut, phi, dphi, x1, x2, y1, y2, c);
+		k1_store_packed(p, ch, x1, x2, y1, y2, phi);
 	}
 }
 
@@ -652,17 +590,9 @@ __global__ void __launch_bounds__(K1L_BLOCK) k1_mix_iir_decimate_lanes(vdl2_k1_p
  * one cp.async.bulk per receiver row, issued by the lanes of warp 0, all completing on the tile's mbarrier.  Each lane
  * reads its receiver's row (the lanes of one receiver broadcast).  The row stride is even, so every row of the plane has
  * the same 16-byte phase and one `mis` serves all of them.  Block shape, NCO table copies and per-lane arithmetic
- * (k1_packed_step, the software-pipelined group body, the symmetric-tap form) are those of the packed kernel, so every
- * decimated sample is the reference's bit for bit.
+ * (k1_sample_loop, the group body of k1_group) are those of the packed kernel, so every decimated sample is the
+ * reference's bit for bit.
  * ---------------------------------------------------------------------------------------------- */
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-	asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_copy(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-			:: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
 template<int OS, bool SYM>
 __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_groups(vdl2_k1_params p) {
 	constexpr int NLUT = 8, LA = 10, MA = 5;
@@ -686,25 +616,15 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_groups(v
 	const float4 *lut = s_lut + (tid & (NLUT - 1));
 	const uint32_t lane_bytes = (tid & (NLUT - 1)) * 16u;
 	if(tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
-	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
+	u64 x1, x2, y1, y2;
 	uint32_t phi = 0, dphi = 0;
-	if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
-	u64 x1 = f2_pack(xr1, xi1), x2 = f2_pack(xr2, xi2), y1 = f2_pack(yr1, yi1), y2 = f2_pack(yr2, yi2);
-	k1_packed_consts c;
-	c.ONE = f2_pack(p.one, p.one); c.SGN = f2_pack(p.neg_one, p.one);
-	c.A0 = f2_pack(p.a0, p.a0); c.A1 = f2_pack(p.a1, p.a1); c.A2 = f2_pack(p.a2, p.a2);
-	c.B1 = f2_pack(p.b1, p.b1); c.B2 = f2_pack(p.b2, p.b2); c.TWO = f2_pack(p.two, p.two);
-	c.one = p.one; c.neg_one = p.neg_one;
+	k1_load_packed(p, ch, active, x1, x2, y1, y2, phi, dphi);
+	const k1_packed_consts c = k1_consts(p, p.a0, p.a1, p.a2, p.b1, p.b2);
 	__syncthreads();
 
 	uint32_t cnt = cnt0, m = 0, pos = 0;
 	const uint32_t head = min(n_pairs, (OS - cnt0 % OS) % OS);
-	if(active) {
-		for(; pos < head; pos++) {
-			u64 y0 = k1_packed_step(samples[pos], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
-			if(++cnt == OS) { cnt = 0; p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0)); m++; }
-		}
-	}
+	if(active) k1_sample_loop<OS, NLUT>(p, ch, samples, 1, 0, pos, head, cnt, m, lut, phi, dphi, x1, x2, y1, y2, c);
 	pos = head;
 	m = (cnt0 + head) / OS;
 	cnt = (cnt0 + head) % OS;
@@ -736,6 +656,8 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_groups(v
 		mbar_wait(&s_bar[tile & 1u], (tile >> 1) & 1u);
 		if(active) {
 			for(uint32_t g = 0; g < ng; g++) {
+				/* k1_group's body, restated: with the call this kernel's schedule changed and it measured 5 % slower
+				 * (DESIGN.md, K1 receiver groups) */
 				const float2 *sp = &s_tile[g * OS];
 				u64 y0 = 0;
 				float2 S[OS];
@@ -783,11 +705,8 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_groups(v
 	};
 	if(mis) tile_loop(std::integral_constant<int, 1>{}); else tile_loop(std::integral_constant<int, 0>{});
 	if(active) {
-		for(; pos < n_pairs; pos++) {
-			u64 y0 = k1_packed_step(samples[pos], lut[((phi >> 16) & 0xFFu) * NLUT], phi, dphi, x1, x2, y1, y2, c);
-			if(++cnt == OS) { cnt = 0; p.dec[(size_t)m * p.n_chp + ch] = make_float2(f2_lo(y0), f2_hi(y0)); m++; }
-		}
-		k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+		k1_sample_loop<OS, NLUT>(p, ch, samples, 1, 0, pos, n_pairs, cnt, m, lut, phi, dphi, x1, x2, y1, y2, c);
+		k1_store_packed(p, ch, x1, x2, y1, y2, phi);
 	}
 	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);
 }
@@ -804,50 +723,13 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_groups(v
  * belong to receivers of different rates run the arms one after the other: correct, but listing the receivers grouped by
  * rate keeps every warp (except at most two per rate boundary) on one arm.
  * ---------------------------------------------------------------------------------------------- */
-/* ng decimation groups of one lane from its staged row: the software-pipelined group body of k1_mix_iir_decimate_groups,
- * operation for operation (k1_packed_step's arithmetic, no contraction, the same rounding order) */
+/* ng decimation groups of one lane from its staged row, decimated sample g to dec[g * n_chp] */
 template<int OS, bool SYM>
 __device__ __forceinline__ void k1m_groups(const float2 *s_row, uint32_t ng, float2 *dec, uint32_t n_chp, const float4 *s_lut,
 		uint32_t lane_bytes, uint32_t &phi, const uint32_t dphi, u64 &x1, u64 &x2, u64 &y1, u64 &y2, u64 &P1, u64 &P2,
 		const k1_packed_consts &c) {
-	constexpr int NLUT = 8, LA = 10, MA = 5;
 	for(uint32_t g = 0; g < ng; g++) {
-		const float2 *sp = &s_row[g * OS];
-		u64 y0 = 0;
-		float2 S[OS];
-		float4 E[OS];
-		float FR[OS];
-		u64 X0[OS];
-#pragma unroll
-		for(int k = -LA; k < OS; k++) {
-			const int kl = k + LA, km = k + MA;
-			if(kl < OS) {
-				const uint32_t ph = phi + (uint32_t)kl * dphi;
-				E[kl] = k1_lut_entry<NLUT>(s_lut, ph, lane_bytes);
-				FR[kl] = (float)(ph & 0xFFFFu);
-				S[kl] = sp[kl];
-			}
-			if(km >= 0 && km < OS) {
-				const u64 CS = f2_fma(f2_mul(f2_pack(E[km].z, E[km].w), f2_pack(FR[km], FR[km])), c.ONE, f2_pack(E[km].x, E[km].y));
-				X0[km] = k1_mix(S[km], CS, c);
-			}
-			if(k >= 0) {
-				const u64 x0 = X0[k];
-				u64 r;
-				if(SYM) {
-					const u64 P0 = f2_mul(c.A0, x0);
-					r = f2_fma(P0, c.ONE, f2_fma(P1, c.TWO, P2));
-					P2 = P1; P1 = P0;
-				} else {
-					const u64 t = f2_fma(f2_mul(c.A1, x1), c.ONE, f2_mul(c.A2, x2));
-					r = f2_fma(f2_mul(c.A0, x0), c.ONE, t);
-				}
-				const u64 u = f2_fma(f2_mul(c.B1, y1), c.ONE, f2_mul(c.B2, y2));
-				y0 = f2_fma(r, c.ONE, u);
-				x2 = x1; x1 = x0; y2 = y1; y1 = y0;
-			}
-		}
-		phi += (uint32_t)OS * dphi;
+		const u64 y0 = k1_group<OS, 8, 1, SYM>(&s_row[g * OS], s_lut, lane_bytes, phi, dphi, x1, x2, y1, y2, P1, P2, c);
 		dec[(size_t)g * n_chp] = make_float2(f2_lo(y0), f2_hi(y0));
 	}
 }
@@ -893,18 +775,12 @@ __device__ __forceinline__ void k1_mixed_body(const vdl2_k1_params &p) {
 	for(uint32_t i = tid; i < 257 * NLUT; i += VDL2_RX_K1_BLOCK) s_lut[i] = p.lut[i / NLUT];
 	const uint32_t lane_bytes = (tid & (NLUT - 1)) * 16u;
 	if(tid == 0) { mbar_init(&s_bar[0], 1); mbar_init(&s_bar[1], 1); mbar_fence_init(); }
-	float xr1 = 0, xr2 = 0, xi1 = 0, xi2 = 0, yr1 = 0, yr2 = 0, yi1 = 0, yi2 = 0;
+	u64 x1, x2, y1, y2;
 	uint32_t phi = 0, dphi = 0;
 	if(RAGGED && fresh) dphi = p.rx_restart[ch].dphi;                         /* (the other fields stay 0) */
-	else if(active) k1_load_state(p, ch, xr1, xr2, xi1, xi2, yr1, yr2, yi1, yi2, phi, dphi);
-	u64 x1 = f2_pack(xr1, xi1), x2 = f2_pack(xr2, xi2), y1 = f2_pack(yr1, yi1), y2 = f2_pack(yr2, yi2);
+	k1_load_packed(p, ch, active && !(RAGGED && fresh), x1, x2, y1, y2, phi, dphi);
 	auto tap = [&](int j) { return cls == 0 ? p.cls_taps[0][j] : cls == 1 ? p.cls_taps[1][j] : p.cls_taps[2][j]; };
-	const float a0 = tap(0), a1 = tap(1), a2 = tap(2), b1 = tap(3), b2 = tap(4);
-	k1_packed_consts c;
-	c.ONE = f2_pack(p.one, p.one); c.SGN = f2_pack(p.neg_one, p.one);
-	c.A0 = f2_pack(a0, a0); c.A1 = f2_pack(a1, a1); c.A2 = f2_pack(a2, a2);
-	c.B1 = f2_pack(b1, b1); c.B2 = f2_pack(b2, b2); c.TWO = f2_pack(p.two, p.two);
-	c.one = p.one; c.neg_one = p.neg_one;
+	const k1_packed_consts c = k1_consts(p, tap(0), tap(1), tap(2), tap(3), tap(4));
 	__syncthreads();
 
 	u64 P1 = f2_mul(c.A0, x1), P2 = f2_mul(c.A0, x2);
@@ -945,7 +821,7 @@ __device__ __forceinline__ void k1_mixed_body(const vdl2_k1_params &p) {
 		if(tid < 32 && tile + 2 < n_tiles) request_tile(tile + 2, tile & 1u);
 	}
 	if(active || (RAGGED && fresh))
-		k1_store_state(p, ch, f2_lo(x1), f2_lo(x2), f2_hi(x1), f2_hi(x2), f2_lo(y1), f2_lo(y2), f2_hi(y1), f2_hi(y2), phi);
+		k1_store_packed(p, ch, x1, x2, y1, y2, phi);
 	if(RAGGED && fresh) p.state[K1_DPHI * p.n_chp + ch] = dphi;
 	if(tid == 0) vdl2_trace_end(p.trace_blocks, trace_k);
 }
@@ -1567,12 +1443,6 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		vdl2_set_carveout(k1_mix_iir_decimate_packed<20, K1_BLOCK1, 10, false>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_packed<10, K1_BLOCK1, 10, true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_packed<10, K1_BLOCK1, 10, false>, pct);
-		vdl2_set_carveout(k1_mix_iir_decimate_packed<20, K1_BLOCK, 10, true, true>, pct);
-		vdl2_set_carveout(k1_mix_iir_decimate_packed<20, K1_BLOCK, 10, false, true>, pct);
-		vdl2_set_carveout(k1_mix_iir_decimate_packed<10, K1_BLOCK, 10, true, true>, pct);
-		vdl2_set_carveout(k1_mix_iir_decimate_packed<10, K1_BLOCK, 10, false, true>, pct);
-		vdl2_set_carveout(k1_mix_iir_decimate_packed<13, K1_BLOCK, 10, true, true>, pct);
-		vdl2_set_carveout(k1_mix_iir_decimate_packed<13, K1_BLOCK, 10, false, true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_scalar<K1_BLOCK1>, pct);
 		vdl2_set_carveout(k0_convert, pct);
 		vdl2_set_carveout(k0_convert_lanes, pct);
@@ -1656,20 +1526,9 @@ extern "C" int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2
 template<int OS, int BLOCK>
 static void k1_launch_packed(const vdl2_k1_params *p, int variant, bool sym, cudaStream_t st) {
 	const uint32_t blocks = (p->n_chp + BLOCK - 1) / BLOCK;
-	if(BLOCK == K1_BLOCK && variant != 0 && p->phase != nullptr) {            /* fused phase pass */
-		if(sym) k1_mix_iir_decimate_packed<OS, K1_BLOCK, 10, true, true><<<blocks, K1_BLOCK, 0, st>>>(*p);
-		else k1_mix_iir_decimate_packed<OS, K1_BLOCK, 10, false, true><<<blocks, K1_BLOCK, 0, st>>>(*p);
-		return;
-	}
 	if(variant == 0 && BLOCK == K1_BLOCK) k1_mix_iir_decimate_packed<OS, K1_BLOCK, 0, false><<<blocks, BLOCK, 0, st>>>(*p);
 	else if(sym) k1_mix_iir_decimate_packed<OS, BLOCK, 10, true><<<blocks, BLOCK, 0, st>>>(*p);
 	else k1_mix_iir_decimate_packed<OS, BLOCK, 10, false><<<blocks, BLOCK, 0, st>>>(*p);
-}
-
-extern "C" int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, int force_scalar, int variant, int receivers) {
-	if(receivers || force_scalar || variant == 0 || variant == 8 || ch_per_stream == 1) return 0;
-	if(ch_per_stream != 0 && ch_per_stream % K1_BLOCK != 0) return 0;
-	return oversample == 20 || oversample == 10 || oversample == 13;
 }
 
 /* variant: 0 un-pipelined packed kernel, 4 no symmetric-tap specialisation, 8 one warp per block (single NCO table copy),

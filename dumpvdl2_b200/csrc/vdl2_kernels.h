@@ -50,12 +50,6 @@ typedef struct {
 	uint32_t stream_stride;      /* float2 elements between consecutive streams in `samples` (ch_per_stream == 1: per sample row) */
 	const vdl2_chunk_args *ca;   /* NULL, or device pointer overriding n_pairs / cnt0 */
 	vdl2_block_trace *trace_blocks;
-	/* fused phase pass (vdl2_k1_fuses_phase): K1 also writes fl32(atan2(im, re)) of every decimated sample to
-	 * phase[(160 + m) * n_chp + slot] and first copies the 160 history rows from phase_prev[(prev_n_dec + i) * n_chp + slot];
-	 * NULL = decimated samples only (a K2a launch produces the phase plane) */
-	float *phase;
-	const float *phase_prev;
-	uint32_t prev_n_dec;         /* overridden by ca->prev_n_dec */
 	/* multi-receiver context (vdl2gpu_create_receivers; NULL otherwise): `samples` is float2[n_rx][stream_stride], receiver-major;
 	 * slot_rx[slot] = receiver of the slot's channel, block_rx[2 b] / [2 b + 1] = first receiver / number of receivers of
 	 * 128-slot block b (vdl2_rx_layout); every tile stages rx_tile samples of each of them, at most rx_max per block */
@@ -163,9 +157,6 @@ int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *r
 int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
 		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
 int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st);
-/* whether vdl2_launch_k1 with these arguments runs a kernel that honours p->phase (the pipelined packed kernel with
- * 128-channel blocks); everything else, the receiver-group kernel included, leaves the phase plane to K2a */
-int vdl2_k1_fuses_phase(uint32_t oversample, uint32_t ch_per_stream, int force_scalar, int variant, int receivers);
 int vdl2_launch_copy_hist(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k2a(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k2a_warps(const vdl2_k2a_params *p, cudaStream_t st);

@@ -83,9 +83,12 @@ def fleet():
     return rxs, spans, pos, oracles, first
 
 
-@pytest.mark.parametrize("flags", [0, vd.FLAG_NO_GRAPH, vd.FLAG_TRACE], ids=["graphs", "no_graph", "trace"])
-def test_ragged_spans_match_the_oracle_per_receiver(fleet, flags):
+@pytest.mark.parametrize("flags,k1_variant", [(0, None), (vd.FLAG_NO_GRAPH, None), (vd.FLAG_TRACE, None), (0, "4")],
+                         ids=["graphs", "no_graph", "trace", "k1_variant4"])
+def test_ragged_spans_match_the_oracle_per_receiver(fleet, flags, k1_variant, monkeypatch):
     rxs, spans, pos, oracles, first = fleet
+    if k1_variant:                                  # without the symmetric-tap form of the filter (read at create)
+        monkeypatch.setenv("VDL2GPU_K1_VARIANT", k1_variant)
     res = _run(rxs, spans, flags, pace=(flags == 0))
     st = res["stats"]
     assert st["pool_overflows"] == 0 and st["out_overflows"] == 0

@@ -212,7 +212,7 @@ def test_cuda_graph_replay_equals_direct_launches():
     assert len(f_graph) > 20
 
 
-@pytest.mark.parametrize("env", [dict(VDL2GPU_K2A=0), dict(VDL2GPU_FUSE_PHASE=1), dict(VDL2GPU_K2_VARIANT=1), dict(VDL2GPU_K2_VARIANT=3),
+@pytest.mark.parametrize("env", [dict(VDL2GPU_K2A=0), dict(VDL2GPU_STAGES=3), dict(VDL2GPU_K2_VARIANT=1), dict(VDL2GPU_K2_VARIANT=3),
                                  dict(VDL2GPU_K2_VARIANT=4), dict(VDL2GPU_K2_VARIANT=5), dict(VDL2GPU_K2_VARIANT=0), dict(VDL2GPU_K1_VARIANT=0),
                                  dict(VDL2GPU_K1_VARIANT=8),
                                  dict(VDL2GPU_K1_VARIANT=4)])
@@ -266,13 +266,13 @@ def test_independent_streams_mode():
     g.close()
 
 
-@pytest.mark.parametrize("n_streams", [32, 40])
-def test_one_stream_per_channel_mode(n_streams):
+@pytest.mark.parametrize("n_streams,os_", [(32, 20), (40, 20), (40, 10)], ids=["32", "40", "40-os10"])
+def test_one_stream_per_channel_mode(n_streams, os_):
     """n_streams == n_channels: every channel demodulates its OWN IQ stream (the reference's traffic model, one buffer
     per channel thread); K0 lays the samples out time-major across streams and K1 runs one lane per stream.  Each
     channel must equal the oracle run on its stream alone; 40 streams leave 24 lanes of the second warp idle."""
     from dumpvdl2_b200 import synth
-    fs, center, chunk = 2100000, cases.CENTER, 131072
+    fs, center, chunk = 105000 * os_, cases.CENTER, 131072
     base, offs, _ = synth.traffic_stream(fs, 0.6, 8, 8.0, 24.0, -20.0, 0x56444C50, "u8")
     n = (base.size // chunk) * chunk
     base = base[:n]
@@ -280,10 +280,10 @@ def test_one_stream_per_channel_mode(n_streams):
     for s in range(n_streams):
         iq = np.roll(base, 2 * 7919 * s)                     # the same traffic, shifted in time: a different stream per channel
         f = center + int(offs[s % len(offs)])
-        o = po.Oracle(fs, 20, po.FMT_U8, center, [f])
+        o = po.Oracle(fs, os_, po.FMT_U8, center, [f])
         o.process_chunked(iq, chunk)
         streams.append(iq); freqs.append(f); want.append(o)
-    g = vd.Vdl2Channels(fs, 20, vd.FMT_U8, center, freqs, max_chunk_bytes=chunk, n_streams=n_streams)
+    g = vd.Vdl2Channels(fs, os_, vd.FMT_U8, center, freqs, max_chunk_bytes=chunk, n_streams=n_streams)
     for off in range(0, n, chunk):
         g.process_buf_uchar(np.concatenate([x[off:off + chunk] for x in streams]))
     got = g.flush()

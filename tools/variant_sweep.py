@@ -89,7 +89,7 @@ def main():
     args = ap.parse_args()
     chunks, offs, _ = bench.make_stream(4.0)
     d_chunks = torch.from_numpy(chunks).cuda()
-    variants = [("default", {}, 0), ("no_graph", {}, vd.FLAG_NO_GRAPH), ("k1_fused_phase", dict(VDL2GPU_FUSE_PHASE=1), 0), ("k2a_libm", dict(VDL2GPU_K2A=0), 0),
+    variants = [("default", {}, 0), ("no_graph", {}, vd.FLAG_NO_GRAPH), ("k2a_libm", dict(VDL2GPU_K2A=0), 0),
                 ("k2_plane", dict(VDL2GPU_K2_VARIANT=2), 0), ("k2_ring_cpasync", dict(VDL2GPU_K2_VARIANT=4), 0),
                 ("k2_ring_staged", dict(VDL2GPU_K2_VARIANT=5), 0), ("k1_one_warp", dict(VDL2GPU_K1_VARIANT=8), 0),
                 ("k2_staged_1warp", dict(VDL2GPU_K2_VARIANT=261), 0), ("k2_plane_1warp", dict(VDL2GPU_K2_VARIANT=258), 0),
