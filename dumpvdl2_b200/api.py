@@ -92,6 +92,7 @@ def load_library():
     L.vdl2gpu_submit_ragged_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.vdl2gpu_get_receiver_positions.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_restart_receiver.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+    L.vdl2gpu_update_receivers.argtypes = [C.c_void_p, C.POINTER(_ReceiverEx), C.c_void_p, C.c_uint32, C.c_void_p]
     L.vdl2gpu_destroy.argtypes = [C.c_void_p]
     L.vdl2gpu_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
@@ -420,7 +421,8 @@ class Vdl2MixedReceivers(Vdl2Receivers):
     With ragged=True the receivers do not advance in lock step: submit_ragged() takes whatever whole decimation groups each
     receiver has (any count, 0 included, per receiver and per span), and every receiver still decodes exactly what one
     reference process decodes from the concatenation of its buffers.  restart_receiver() starts one receiver afresh (a
-    reconnect, a swapped device, a retune) without disturbing the others."""
+    reconnect, a swapped device, a retune) without disturbing the others, and update_receivers() / add_receivers() /
+    remove_receivers() let receivers join and leave (after flush()) while the others carry on."""
 
     def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, ragged=False):
         """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16))"""
@@ -428,19 +430,10 @@ class Vdl2MixedReceivers(Vdl2Receivers):
             flags |= FLAG_RAGGED
         self.ragged = bool(flags & FLAG_RAGGED)
         self.L = load_library()
-        rxs = [(int(cf), [int(f) for f in fr], int(os_), int(fmt)) for cf, fr, os_, fmt in receivers]
-        self.receivers = [(cf, fr) for cf, fr, _, _ in rxs]
-        self.oversample = [os_ for _, _, os_, _ in rxs]
-        self.formats = [fmt for _, _, _, fmt in rxs]
-        self.bytes_per_dec = [os_ * (4 if fmt == FMT_S16 else 2) for _, _, os_, fmt in rxs]
-        self.n_receivers = self.n_streams = len(rxs)
-        self.freqs = np.ascontiguousarray([f for _, fr in self.receivers for f in fr], dtype=np.uint32)
-        self.n_channels = int(self.freqs.size)
-        self._first = np.concatenate([[0], np.cumsum([len(fr) for _, fr in self.receivers], dtype=np.int64)]).astype(np.int64)
+        rxs = self._normalise(receivers)
+        self._describe(rxs)
         self.sample_fmt = None
-        rx = (_ReceiverEx * max(self.n_receivers, 1))()
-        for r, (cf, fr, os_, fmt) in enumerate(rxs):
-            rx[r].centerfreq, rx[r].n_channels, rx[r].oversample, rx[r].sample_fmt = cf, len(fr), os_, fmt
+        rx = self._c_receivers(rxs)
         cfg = _Config()                              # sample_rate, oversample, sample_fmt and centerfreq stay 0: per receiver
         cfg.n_channels = self.n_channels
         cfg.freqs = self.freqs.ctypes.data_as(C.POINTER(C.c_uint32))
@@ -451,6 +444,28 @@ class Vdl2MixedReceivers(Vdl2Receivers):
                "vdl2gpu_create_mixed_receivers")
         self._frames = []
         self._cb = _FRAME_CB(self._on_frame)
+
+    @staticmethod
+    def _normalise(receivers):
+        return [(int(cf), [int(f) for f in fr], int(os_), int(fmt)) for cf, fr, os_, fmt in receivers]
+
+    def _describe(self, rxs):
+        """the per-receiver attributes of the list rxs of (centre, [freqs], oversample, format)"""
+        self.receivers = [(cf, fr) for cf, fr, _, _ in rxs]
+        self.oversample = [os_ for _, _, os_, _ in rxs]
+        self.formats = [fmt for _, _, _, fmt in rxs]
+        self.bytes_per_dec = [os_ * (4 if fmt == FMT_S16 else 2) for _, _, os_, fmt in rxs]
+        self.n_receivers = self.n_streams = len(rxs)
+        self.freqs = np.ascontiguousarray([f for _, fr in self.receivers for f in fr], dtype=np.uint32)
+        self.n_channels = int(self.freqs.size)
+        self._first = np.concatenate([[0], np.cumsum([len(fr) for _, fr in self.receivers], dtype=np.int64)]).astype(np.int64)
+
+    @staticmethod
+    def _c_receivers(rxs):
+        rx = (_ReceiverEx * max(len(rxs), 1))()
+        for r, (cf, fr, os_, fmt) in enumerate(rxs):
+            rx[r].centerfreq, rx[r].n_channels, rx[r].oversample, rx[r].sample_fmt = cf, len(fr), os_, fmt
+        return rx
 
     def _submit(self, buf, fmt):
         raise Vdl2GpuError("a mixed-receivers context takes spans of decimated samples: use submit_span / submit_span_device")
@@ -547,3 +562,59 @@ class Vdl2MixedReceivers(Vdl2Receivers):
                 span.append(p[pos[r] * w:(pos[r] + n) * w])
                 pos[r] += n
             self.submit_ragged(span)
+
+    # ---- receivers joining and leaving (ragged=True) ----
+    def update_receivers(self, receivers, from_):
+        """Replace the receiver list with `receivers` [(centerfreq, [freqs...], oversample, fmt), ...] on a drained context
+        (flush() first).  from_[i] is the current index of the receiver entry i continues, which it must describe exactly
+        as it is now (receivers[k], oversample[k], formats[k]), or -1 for a new receiver; receivers not named are removed.
+        Kept receivers carry on undisturbed under their new indices and channel numbers; a new one starts as a freshly
+        started reference process.  Read a receiver's counters before removing it."""
+        rxs = self._normalise(receivers)
+        src = [int(k) for k in from_]
+        if len(src) != len(rxs):
+            raise ValueError(f"{len(src)} entries in from_ for {len(rxs)} receivers")
+        if not rxs:
+            raise ValueError("no receivers")
+        seen = set()
+        for i, k in enumerate(src):
+            if k == -1:
+                continue
+            if not 0 <= k < self.n_receivers:
+                raise ValueError(f"entry {i} continues receiver {k} of {self.n_receivers}")
+            if k in seen:
+                raise ValueError(f"entry {i} continues receiver {k}, which an earlier entry continues")
+            seen.add(k)
+            cf, fr = self.receivers[k]
+            if rxs[i] != (cf, list(fr), self.oversample[k], self.formats[k]):
+                raise ValueError(f"entry {i} does not repeat receiver {k}'s description (retune with restart_receiver)")
+        rx = self._c_receivers(rxs)
+        fr = np.ascontiguousarray([f for _, fl, _, _ in rxs for f in fl], dtype=np.uint32)
+        fa = np.ascontiguousarray(src, dtype=np.int32)
+        _check(self.L, self.L.vdl2gpu_update_receivers(self.h, rx, fa.ctypes.data, len(rxs), fr.ctypes.data), "vdl2gpu_update_receivers")
+        self._describe(rxs)
+
+    def _current(self, k):
+        cf, fr = self.receivers[k]
+        return (cf, list(fr), self.oversample[k], self.formats[k])
+
+    def add_receivers(self, receivers, at=None):
+        """insert new receivers before index `at` (None: at the end); every receiver from `at` on moves up"""
+        new = self._normalise(receivers)
+        at = self.n_receivers if at is None else int(at)
+        if not 0 <= at <= self.n_receivers:
+            raise ValueError(f"position {at} of {self.n_receivers} receivers")
+        old = list(range(self.n_receivers))
+        self.update_receivers([self._current(k) for k in old[:at]] + new + [self._current(k) for k in old[at:]],
+                              old[:at] + [-1] * len(new) + old[at:])
+
+    def remove_receivers(self, indices):
+        """remove the receivers at these indices; the others keep their order and move down"""
+        gone = set()
+        for k in indices:
+            k = int(k)
+            if not 0 <= k < self.n_receivers:
+                raise ValueError(f"receiver {k} of {self.n_receivers}")
+            gone.add(k)
+        keep = [k for k in range(self.n_receivers) if k not in gone]
+        self.update_receivers([self._current(k) for k in keep], keep)

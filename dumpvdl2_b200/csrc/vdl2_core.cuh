@@ -1351,4 +1351,49 @@ typedef struct {
 	uint32_t restart, dphi, freq;
 } vdl2_rx_restart;
 
+/* ------------------------------------------------------------------------------------------------
+ * Receivers joining and leaving a ragged context (vdl2gpu_update_receivers): the new receiver list rx[0..n_rx) names, per
+ * entry, the old receiver it continues (from[r] >= 0) or none (from[r] == -1, a new receiver).  A kept receiver repeats its
+ * description, so its channel k is old channel old_first[from[r]] + k; each kept channel carries its whole state from
+ * its old slot to its new one, and a new receiver's channels start as create starts them.
+ * ---------------------------------------------------------------------------------------------- */
+/* channel -> slot, the inverse of vdl2_slot_channel */
+VDL2_HD uint32_t vdl2_channel_slot(uint32_t ch, uint32_t lanes, uint32_t full_warps) {
+	const uint32_t head = full_warps * lanes;
+	if(ch < head) return (ch / lanes) * 32u + ch % lanes;
+	const uint32_t c = ch - head;
+	return (full_warps + c / (lanes - 1u)) * 32u + c % (lanes - 1u);
+}
+
+/* the old channel new channel `chan` continues, or -1 (a channel of a new receiver); rx_first[n_rx + 1] are the new
+ * receivers' first channels, old_first those of the old list */
+VDL2_HD int32_t vdl2_rx_chan_from(uint32_t chan, const uint32_t *rx_first, uint32_t n_rx, const int32_t *from, const uint32_t *old_first) {
+	const uint32_t r = vdl2_rx_of_channel(chan, rx_first, n_rx);
+	if(from[r] < 0) return -1;
+	return (int32_t)(old_first[from[r]] + (chan - rx_first[r]));
+}
+
+#define VDL2_MIGRATE_FRESH (-1)                /* the slot's channel belongs to a new receiver */
+#define VDL2_MIGRATE_NONE (-2)                 /* the slot holds no channel */
+
+/* The old slot new slot `slot` continues (new layout: lanes, full_warps, n_ch, rx_first; old layout: old_lanes,
+ * old_full_warps, old_first), VDL2_MIGRATE_FRESH or VDL2_MIGRATE_NONE.  Each kept channel maps to its own old slot and
+ * nothing else maps to an old slot, since from[] names each old receiver at most once. */
+VDL2_HD int32_t vdl2_rx_slot_from(uint32_t slot, uint32_t lanes, uint32_t full_warps, uint32_t n_ch, const uint32_t *rx_first,
+		uint32_t n_rx, const int32_t *from, uint32_t old_lanes, uint32_t old_full_warps, const uint32_t *old_first) {
+	uint32_t chan;
+	if(!vdl2_slot_channel(slot, lanes, full_warps, n_ch, chan)) return VDL2_MIGRATE_NONE;
+	const int32_t old = vdl2_rx_chan_from(chan, rx_first, n_rx, from, old_first);
+	return old < 0 ? VDL2_MIGRATE_FRESH : (int32_t)vdl2_channel_slot((uint32_t)old, old_lanes, old_full_warps);
+}
+
+/* entry i of the migration table: slot i of the new planes and channel i of the new counters (the counters are kept by
+ * channel, the state by slot) */
+typedef struct {
+	int32_t slot_from;           /* slot i: vdl2_rx_slot_from */
+	uint32_t hist_row;           /* ... kept: its receiver's count in the last span (prev_n), where its last 160 phases start */
+	uint32_t dphi, freq;         /* ... fresh: NCO step (vdl2_nco_dphi) and frequency */
+	int32_t chan_from;           /* channel i: the old channel whose counters it continues, or -1 (zero counters) */
+} vdl2_rx_migrate;
+
 #endif

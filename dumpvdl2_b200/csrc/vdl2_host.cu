@@ -159,12 +159,7 @@ struct vdl2gpu_ctx {
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
 		uint32_t n_chp, uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2);
 /* channel -> slot: the first full_warps warps hold `lanes` channels each, the others lanes - 1 */
-static inline uint32_t slot_of(uint32_t ch, uint32_t lanes, uint32_t full_warps) {
-	const uint32_t head = full_warps * lanes;
-	if(ch < head) return (ch / lanes) * 32u + ch % lanes;
-	const uint32_t c = ch - head;
-	return (full_warps + c / (lanes - 1u)) * 32u + c % (lanes - 1u);
-}
+static inline uint32_t slot_of(uint32_t ch, uint32_t lanes, uint32_t full_warps) { return vdl2_channel_slot(ch, lanes, full_warps); }
 
 extern "C" int vdl2gpu_abi_version(void) { return VDL2GPU_ABI_VERSION; }
 
@@ -189,12 +184,8 @@ extern "C" const char *vdl2gpu_strerror(int code) {
 	}
 }
 
-static int free_ctx(vdl2gpu_ctx *c) {
-	if(!c) return VDL2GPU_OK;
-	cudaSetDevice(c->device);
-	if(c->stream) cudaStreamSynchronize(c->stream);
-	if(c->s_mid) cudaStreamSynchronize(c->s_mid);
-	if(c->s_back) cudaStreamSynchronize(c->s_back);
+/* the device buffers and chunk slots of setup_layout (nothing may be running on them) */
+static void free_layout(vdl2gpu_ctx *c) {
 	for(auto &s : c->chunks) {
 		if(s.h_raw) cudaFreeHost(s.h_raw);
 		if(s.d_raw) cudaFree(s.d_raw);
@@ -213,14 +204,24 @@ static int free_ctx(vdl2gpu_ctx *c) {
 		if(s.h_restart) cudaFreeHost(s.h_restart);
 		if(s.d_restart) cudaFree(s.d_restart);
 	}
-	cudaFree(c->d_tab); cudaFree(c->d_samples);
+	c->chunks.clear();
+	cudaFree(c->d_samples);
 	for(int i = 0; i < 3; i++) cudaFree(c->d_dec3[i]);
 	for(int i = 0; i < 2; i++) { cudaFree(c->d_phase2[i]); cudaFree(c->d_mag2[i]); }
 	cudaFree(c->d_k1); cudaFree(c->d_k2);
-	cudaFree(c->d_counters); cudaFree(c->d_ready); cudaFree(c->d_ring); cudaFree(c->d_pool); cudaFree(c->d_free);
-	cudaFree(c->d_ctl); cudaFree(c->d_events); cudaFree(c->d_block_trace);
+	cudaFree(c->d_counters); cudaFree(c->d_ready); cudaFree(c->d_ring); cudaFree(c->d_pool); cudaFree(c->d_free); cudaFree(c->d_ctl);
 	cudaFree(c->d_slot_rx); cudaFree(c->d_block_rx);
 	cudaFree(c->d_rx_in); cudaFree(c->d_slot_cls);
+}
+
+static int free_ctx(vdl2gpu_ctx *c) {
+	if(!c) return VDL2GPU_OK;
+	cudaSetDevice(c->device);
+	if(c->stream) cudaStreamSynchronize(c->stream);
+	if(c->s_mid) cudaStreamSynchronize(c->s_mid);
+	if(c->s_back) cudaStreamSynchronize(c->s_back);
+	free_layout(c);
+	cudaFree(c->d_tab); cudaFree(c->d_events); cudaFree(c->d_block_trace);
 	if(c->ev_input_ready) cudaEventDestroy(c->ev_input_ready);
 	if(c->ev_input_consumed) cudaEventDestroy(c->ev_input_consumed);
 	if(c->ev_drain) cudaEventDestroy(c->ev_drain);
@@ -232,6 +233,193 @@ static int free_ctx(vdl2gpu_ctx *c) {
 	if(c->stream) cudaStreamDestroy(c->stream);
 	delete c;
 	return VDL2GPU_OK;
+}
+
+/* The part of a context that follows from its channels and receivers: the channel slot mapping, span and chunk sizes,
+ * burst-pool size, output capacity, receiver tables, per-receiver host records, and every device buffer and chunk slot
+ * sized by them.  Create and vdl2gpu_update_receivers both build it here, so the two cannot drift apart.  The checks come
+ * first: an EINVAL or ETOOBIG return has touched no device.  The contents of the state planes, the free list and the queue
+ * control block are left to the caller.  c->cfg carries the context's flags, max_chunk_bytes and n_inflight; cfg the
+ * channels (and, for create, the n_streams the caller asked for); rx / n_rx / rx_ex as for create_impl.  The pool holds at
+ * least min_slots slots. */
+static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu_receiver *rx, uint32_t n_rx,
+		const vdl2gpu_receiver_ex *rx_ex, uint32_t min_slots, const char *what) {
+	c->freqs.assign(cfg->freqs, cfg->freqs + cfg->n_channels);
+	c->cfg.freqs = c->freqs.data();
+	c->cfg.n_channels = cfg->n_channels;
+	c->n_ch = cfg->n_channels;
+	c->n_chp = (c->n_ch + 31u) & ~31u;
+	c->lanes = 32; c->full_warps = 0xFFFFFFFFu;
+	/* Slot mapping.  K1 and K2 run four-warp blocks, one warp per SM sub-partition, and a chunk's K2 overlaps the next
+	 * chunk's K1.  The block scheduler places a new block on the SM with the most free resources: when a grid leaves SMs
+	 * empty (128 blocks on 132 SMs at 16384 channels), the OTHER kernel's blocks pile up on those SMs two and three deep
+	 * instead of sitting beside the first kernel's blocks, one per SM, and run two to three times slower (measured with
+	 * the per-block trace, tools/block_trace.py).  So when the channels fill more than half of the machine's
+	 * sub-partitions, they are dealt out evenly over ALL of them: every warp holds floor or ceil of n_ch / (4 x SMs)
+	 * channels instead of 32 (31 or 32 at 16384 channels on 132 SMs), each of the two kernels launches exactly one block
+	 * per SM, every block lives for the whole kernel, and every SM looks the same to the scheduler. */
+	if(c->receivers || cfg->n_streams <= 1 || cfg->n_streams == cfg->n_channels) {
+		const uint32_t warps_all = 4u * (uint32_t)c->n_sms;
+		if(c->n_ch > 16u * warps_all && c->n_ch <= 32u * warps_all) {
+			const char *e = getenv("VDL2GPU_BALANCE");
+			if(!e || atoi(e)) {
+				c->lanes = (c->n_ch + warps_all - 1u) / warps_all;
+				c->full_warps = c->n_ch - (c->lanes - 1u) * warps_all;       /* warps with `lanes` channels; the rest have lanes - 1 */
+				c->n_chp = warps_all * 32u;
+			}
+		}
+	}
+	const uint32_t max_bytes = c->cfg.max_chunk_bytes;
+	if(c->mixed) {
+		/* the largest span: every receiver's buffer within max_chunk_bytes; the plane's row stride holds the longest row */
+		uint32_t bpd_max = 0;
+		for(uint32_t r = 0; r < n_rx; r++) {
+			bpd_max = std::max(bpd_max, rx_ex[r].oversample * (rx_ex[r].sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u));
+			c->rx_os_max = std::max(c->rx_os_max, rx_ex[r].oversample);
+		}
+		c->max_span = max_bytes / bpd_max;
+		if(c->max_span == 0) {
+			snprintf(g_last_error, sizeof(g_last_error), "%s: max_chunk_bytes (%u) holds less than one decimated sample of a receiver (%u bytes)",
+					what, max_bytes, bpd_max);
+			return VDL2GPU_EINVAL;
+		}
+		c->max_pairs = (c->max_span * c->rx_os_max + 1u) & ~1u;       /* even row stride: every row of the plane starts 16-byte aligned */
+		c->max_dec = c->max_span + 2;
+	} else {
+		c->max_pairs = max_bytes / (cfg->sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
+		if(c->receivers) c->max_pairs = (c->max_pairs + 1u) & ~1u;     /* even row stride: every receiver row of the plane starts 16-byte aligned */
+		c->max_dec = c->max_pairs / cfg->oversample + 2;
+	}
+	if((uint64_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp >= (1ull << 32)) {
+		snprintf(g_last_error, sizeof(g_last_error), "%u channels x %u decimated samples per chunk exceed the 32-bit element index of the kernels; "
+				"use a smaller max_chunk_bytes or shard the channels", c->n_ch, c->max_dec);
+		return VDL2GPU_ETOOBIG;
+	}
+	c->n_slots = std::max(std::max(256u, 3u * c->n_ch), min_slots);
+	c->out_cap = std::max(4u << 20, c->n_ch * 512u);
+
+	/* receiver tables (host side) */
+	std::vector<uint32_t> slot_rx, block_rx;
+	std::vector<uint8_t> slot_cls;
+	if(c->receivers) {
+		/* the slot -> receiver tables K1 stages by */
+		std::vector<uint32_t> rx_first(n_rx + 1, 0);
+		for(uint32_t r = 0; r < n_rx; r++) rx_first[r + 1] = rx_first[r] + rx[r].n_channels;
+		const uint32_t n_blocks = (c->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
+		slot_rx.resize((size_t)n_blocks * VDL2_RX_K1_BLOCK); block_rx.resize(2 * (size_t)n_blocks);
+		c->rx_max = vdl2_rx_layout(n_blocks, c->lanes, c->full_warps, c->n_ch, rx_first.data(), n_rx, slot_rx.data(), block_rx.data());
+		c->rx_tile = c->mixed ? vdl2_rx_mixed_tile_groups(c->rx_max, c->rx_os_max) : vdl2_rx_tile_samples(c->rx_max, cfg->oversample);
+		if(c->mixed) {
+			/* per receiver: oversample, format, place in a span; per slot: rate class; per class: the filter taps of
+			 * input_lpf_init(105000 x os) (src/demod.c:367-370) */
+			std::vector<uint32_t> os(n_rx), fmt(n_rx);
+			for(uint32_t r = 0; r < n_rx; r++) { os[r] = rx_ex[r].oversample; fmt[r] = rx_ex[r].sample_fmt; }
+			c->rx_in.resize(n_rx);
+			c->span_bytes_per_dec = vdl2_rx_span_layout(os.data(), fmt.data(), n_rx, c->rx_in.data());
+			for(uint32_t r = 0; r < n_rx; r++) {
+				c->span_pairs_per_dec += os[r];
+				c->cls_mask |= 1u << vdl2_rx_class(os[r]);
+			}
+			static const uint32_t class_os[3] = { 10, 13, 20 };
+			for(int k = 0; k < 3; k++) {
+				float A[3], B[3];
+				make_lpf((uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * class_os[k], A, B);
+				c->cls_taps[k][0] = A[0]; c->cls_taps[k][1] = A[1]; c->cls_taps[k][2] = A[2]; c->cls_taps[k][3] = B[1]; c->cls_taps[k][4] = B[2];
+			}
+			slot_cls.resize(slot_rx.size());
+			for(size_t s = 0; s < slot_rx.size(); s++) slot_cls[s] = (uint8_t)vdl2_rx_class(os[slot_rx[s]]);
+		}
+		if(c->ragged) {
+			c->rx_pos.assign(n_rx, 0);
+			c->rx_prev.assign(n_rx, 0);
+			c->ch_rx.resize(c->n_ch);
+			for(uint32_t r = 0; r < n_rx; r++) std::fill(c->ch_rx.begin() + rx_first[r], c->ch_rx.begin() + rx_first[r + 1], r);
+			c->rx_first = rx_first;
+			c->rx_centre.resize(n_rx);
+			for(uint32_t r = 0; r < n_rx; r++) c->rx_centre[r] = rx[r].centerfreq;
+			c->rx_restart_pending.assign(n_rx, 0);
+			c->n_restart_pending = 0;
+		}
+	}
+
+	/* device buffers */
+	if(c->lane_streams) CU(cudaMalloc(&c->d_samples, (size_t)c->max_pairs * c->n_chp * sizeof(float2)));
+	else CU(cudaMalloc(&c->d_samples, (size_t)c->n_streams * c->max_pairs * sizeof(float2)));
+	for(int i = 0; i < 3; i++) {
+		CU(cudaMalloc(&c->d_dec3[i], (size_t)c->max_dec * c->n_chp * sizeof(float2)));
+		CU(cudaMemset(c->d_dec3[i], 0, (size_t)c->max_dec * c->n_chp * sizeof(float2)));
+	}
+	for(int i = 0; i < 2; i++) {
+		CU(cudaMalloc(&c->d_phase2[i], (size_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp * sizeof(float)));
+		CU(cudaMemset(c->d_phase2[i], 0, (size_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp * sizeof(float)));
+		CU(cudaMalloc(&c->d_mag2[i], (size_t)c->max_dec * c->n_chp * sizeof(float)));
+	}
+	CU(cudaMalloc(&c->d_k1, (size_t)K1_NFIELDS * c->n_chp * 4));
+	CU(cudaMalloc(&c->d_k2, (size_t)K2_NFIELDS * c->n_chp * 4));
+	CU(cudaMalloc(&c->d_counters, (size_t)VDL2_NUM_COUNTERS * c->n_chp * 4));
+	CU(cudaMalloc(&c->d_ring, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
+	CU(cudaMalloc(&c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
+	CU(cudaMalloc(&c->d_free, (size_t)c->n_slots * 4));
+	CU(cudaMalloc(&c->d_ready, (size_t)c->n_slots * 4));
+	CU(cudaMalloc(&c->d_ctl, sizeof(vdl2_queue_ctl)));
+	CU(cudaMemset(c->d_counters, 0, (size_t)VDL2_NUM_COUNTERS * c->n_chp * 4));
+	CU(cudaMemset(c->d_ring, 0, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
+	CU(cudaMemset(c->d_pool, 0, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
+	if(c->receivers) {
+		CU(cudaMalloc(&c->d_slot_rx, slot_rx.size() * 4));
+		CU(cudaMalloc(&c->d_block_rx, block_rx.size() * 4));
+		CU(cudaMemcpy(c->d_slot_rx, slot_rx.data(), slot_rx.size() * 4, cudaMemcpyHostToDevice));
+		CU(cudaMemcpy(c->d_block_rx, block_rx.data(), block_rx.size() * 4, cudaMemcpyHostToDevice));
+	}
+	if(c->mixed) {
+		CU(cudaMalloc(&c->d_rx_in, c->rx_in.size() * sizeof(vdl2_rx_input)));
+		CU(cudaMalloc(&c->d_slot_cls, slot_cls.size()));
+		CU(cudaMemcpy(c->d_rx_in, c->rx_in.data(), c->rx_in.size() * sizeof(vdl2_rx_input), cudaMemcpyHostToDevice));
+		CU(cudaMemcpy(c->d_slot_cls, slot_cls.data(), slot_cls.size(), cudaMemcpyHostToDevice));
+	}
+
+	c->chunks.resize(c->cfg.n_inflight);
+	for(auto &s : c->chunks) {
+		/* h_raw / d_raw (max_chunk_bytes x n_streams each) are allocated by the first vdl2gpu_submit: hosts that only
+		 * use vdl2gpu_submit_device never need them */
+		CU(cudaHostAlloc((void **)&s.h_args, sizeof(vdl2_chunk_args), cudaHostAllocDefault));
+		CU(cudaMalloc(&s.d_args, sizeof(vdl2_chunk_args)));
+		if(c->ragged) {
+			CU(cudaHostAlloc((void **)&s.h_span, (size_t)n_rx * sizeof(vdl2_rx_span), cudaHostAllocDefault));
+			CU(cudaMalloc(&s.d_span, (size_t)n_rx * sizeof(vdl2_rx_span)));
+			CU(cudaHostAlloc((void **)&s.h_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart), cudaHostAllocDefault));
+			CU(cudaMalloc(&s.d_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart)));
+		}
+		CU(cudaHostAlloc((void **)&s.h_out, sizeof(vdl2_out_header) + c->out_cap, cudaHostAllocMapped));
+		CU(cudaHostGetDevicePointer((void **)&s.d_out, s.h_out, 0));
+		memset(s.h_out, 0, sizeof(vdl2_out_header));
+		CU(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+		for(auto &ev : s.tk) CU(cudaEventCreate(&ev));
+	}
+	return VDL2GPU_OK;
+}
+
+/* exchange what setup_layout built (the switch of vdl2gpu_update_receivers) */
+static void swap_layout(vdl2gpu_ctx *a, vdl2gpu_ctx *b) {
+	using std::swap;
+	swap(a->freqs, b->freqs);
+	a->cfg.freqs = a->freqs.data(); b->cfg.freqs = b->freqs.data();
+	swap(a->cfg.n_channels, b->cfg.n_channels); swap(a->cfg.n_streams, b->cfg.n_streams);
+	swap(a->n_ch, b->n_ch); swap(a->n_chp, b->n_chp); swap(a->lanes, b->lanes); swap(a->full_warps, b->full_warps);
+	swap(a->n_streams, b->n_streams);
+	swap(a->max_pairs, b->max_pairs); swap(a->max_dec, b->max_dec); swap(a->max_span, b->max_span);
+	swap(a->n_slots, b->n_slots); swap(a->out_cap, b->out_cap);
+	swap(a->rx_tile, b->rx_tile); swap(a->rx_max, b->rx_max); swap(a->rx_os_max, b->rx_os_max); swap(a->cls_mask, b->cls_mask);
+	swap(a->cls_taps, b->cls_taps);
+	swap(a->rx_in, b->rx_in); swap(a->span_bytes_per_dec, b->span_bytes_per_dec); swap(a->span_pairs_per_dec, b->span_pairs_per_dec);
+	swap(a->rx_pos, b->rx_pos); swap(a->rx_prev, b->rx_prev); swap(a->ch_rx, b->ch_rx);
+	swap(a->rx_centre, b->rx_centre); swap(a->rx_first, b->rx_first);
+	swap(a->rx_restart_pending, b->rx_restart_pending); swap(a->n_restart_pending, b->n_restart_pending);
+	swap(a->d_slot_rx, b->d_slot_rx); swap(a->d_block_rx, b->d_block_rx); swap(a->d_rx_in, b->d_rx_in); swap(a->d_slot_cls, b->d_slot_cls);
+	swap(a->d_samples, b->d_samples); swap(a->d_dec3, b->d_dec3); swap(a->d_phase2, b->d_phase2); swap(a->d_mag2, b->d_mag2);
+	swap(a->d_k1, b->d_k1); swap(a->d_k2, b->d_k2); swap(a->d_counters, b->d_counters); swap(a->d_ring, b->d_ring);
+	swap(a->d_pool, b->d_pool); swap(a->d_free, b->d_free); swap(a->d_ready, b->d_ready); swap(a->d_ctl, b->d_ctl);
+	swap(a->chunks, b->chunks);
 }
 
 /* rx / n_rx: the receivers of a multi-receiver context (vdl2gpu_create_receivers, validated there), NULL / 0 otherwise;
@@ -284,63 +472,12 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 		if((e = getenv("VDL2GPU_K2A_SPLIT")) && atoi(e) >= 1 && atoi(e) <= 256) c->k2a_split = (uint32_t)atoi(e);
 	}
 	if(cfg->flags & (VDL2GPU_FLAG_NO_GRAPH | VDL2GPU_FLAG_TRACE)) c->use_graphs = false;
-	c->freqs.assign(cfg->freqs, cfg->freqs + cfg->n_channels);
-	c->cfg.freqs = c->freqs.data();
-	c->n_ch = cfg->n_channels;
-	c->n_chp = (c->n_ch + 31u) & ~31u;
 	c->n_sms = prop.multiProcessorCount;
-	c->lanes = 32; c->full_warps = 0xFFFFFFFFu;
-	/* Slot mapping.  K1 and K2 run four-warp blocks, one warp per SM sub-partition, and a chunk's K2 overlaps the next
-	 * chunk's K1.  The block scheduler places a new block on the SM with the most free resources: when a grid leaves SMs
-	 * empty (128 blocks on 132 SMs at 16384 channels), the OTHER kernel's blocks pile up on those SMs two and three deep
-	 * instead of sitting beside the first kernel's blocks, one per SM, and run two to three times slower (measured with
-	 * the per-block trace, tools/block_trace.py).  So when the channels fill more than half of the machine's
-	 * sub-partitions, they are dealt out evenly over ALL of them: every warp holds floor or ceil of n_ch / (4 x SMs)
-	 * channels instead of 32 (31 or 32 at 16384 channels on 132 SMs), each of the two kernels launches exactly one block
-	 * per SM, every block lives for the whole kernel, and every SM looks the same to the scheduler. */
-	if(c->receivers || cfg->n_streams <= 1 || cfg->n_streams == cfg->n_channels) {
-		const uint32_t warps_all = 4u * (uint32_t)c->n_sms;
-		if(c->n_ch > 16u * warps_all && c->n_ch <= 32u * warps_all) {
-			const char *e = getenv("VDL2GPU_BALANCE");
-			if(!e || atoi(e)) {
-				c->lanes = (c->n_ch + warps_all - 1u) / warps_all;
-				c->full_warps = c->n_ch - (c->lanes - 1u) * warps_all;       /* warps with `lanes` channels; the rest have lanes - 1 */
-				c->n_chp = warps_all * 32u;
-			}
-		}
-	}
-	const uint32_t max_bytes = cfg->max_chunk_bytes ? cfg->max_chunk_bytes : (1u << 20);
-	c->cfg.max_chunk_bytes = max_bytes;
-	if(c->mixed) {
-		/* the largest span: every receiver's buffer within max_chunk_bytes; the plane's row stride holds the longest row */
-		uint32_t bpd_max = 0;
-		for(uint32_t r = 0; r < n_rx; r++) {
-			bpd_max = std::max(bpd_max, rx_ex[r].oversample * (rx_ex[r].sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u));
-			c->rx_os_max = std::max(c->rx_os_max, rx_ex[r].oversample);
-		}
-		c->max_span = max_bytes / bpd_max;
-		if(c->max_span == 0) {
-			snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_create_mixed_receivers: max_chunk_bytes (%u) holds less than one decimated sample of a receiver (%u bytes)",
-					max_bytes, bpd_max);
-			return VDL2GPU_EINVAL;
-		}
-		c->max_pairs = (c->max_span * c->rx_os_max + 1u) & ~1u;       /* even row stride: every row of the plane starts 16-byte aligned */
-		c->max_dec = c->max_span + 2;
-	} else {
-		c->max_pairs = max_bytes / (cfg->sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
-		if(c->receivers) c->max_pairs = (c->max_pairs + 1u) & ~1u;     /* even row stride: every receiver row of the plane starts 16-byte aligned */
-		c->max_dec = c->max_pairs / cfg->oversample + 2;
-	}
-	if((uint64_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp >= (1ull << 32)) {
-		snprintf(g_last_error, sizeof(g_last_error), "%u channels x %u decimated samples per chunk exceed the 32-bit element index of the kernels; "
-				"use a smaller max_chunk_bytes or shard the channels", c->n_ch, c->max_dec);
-		return VDL2GPU_ETOOBIG;
-	}
-	c->n_slots = std::max(256u, 3u * c->n_ch);
-	c->out_cap = std::max(4u << 20, c->n_ch * 512u);
-	const uint32_t n_inflight = cfg->n_inflight ? cfg->n_inflight : 4u;
-	c->cfg.n_inflight = n_inflight;
+	c->cfg.max_chunk_bytes = cfg->max_chunk_bytes ? cfg->max_chunk_bytes : (1u << 20);
+	c->cfg.n_inflight = cfg->n_inflight ? cfg->n_inflight : 4u;
 	c->event_cap = (cfg->flags & VDL2GPU_FLAG_TRACE) ? (1u << 20) : 1u;
+	int rc = setup_layout(c, cfg, rx, n_rx, rx_ex, 0, c->mixed ? "vdl2gpu_create_mixed_receivers" : c->receivers ? "vdl2gpu_create_receivers" : "vdl2gpu_create");
+	if(rc) return rc;
 	/* (mixed receivers: the rate only enters the filter taps of these tables, which the mixed K1 takes per rate class) */
 	make_tables(c->tab, c->mixed ? (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * c->rx_os_max : cfg->sample_rate);
 	memset(&c->stats, 0, sizeof(c->stats));
@@ -369,80 +506,14 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	}
 	CU(cudaMalloc(&c->d_tab, sizeof(vdl2_tables)));
 	CU(cudaMemcpy(c->d_tab, &c->tab.t, sizeof(vdl2_tables), cudaMemcpyHostToDevice));
-	if(c->lane_streams) CU(cudaMalloc(&c->d_samples, (size_t)c->max_pairs * c->n_chp * sizeof(float2)));
-	else CU(cudaMalloc(&c->d_samples, (size_t)c->n_streams * c->max_pairs * sizeof(float2)));
-	for(int i = 0; i < 3; i++) {
-		CU(cudaMalloc(&c->d_dec3[i], (size_t)c->max_dec * c->n_chp * sizeof(float2)));
-		CU(cudaMemset(c->d_dec3[i], 0, (size_t)c->max_dec * c->n_chp * sizeof(float2)));
-	}
-	for(int i = 0; i < 2; i++) {
-		CU(cudaMalloc(&c->d_phase2[i], (size_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp * sizeof(float)));
-		CU(cudaMemset(c->d_phase2[i], 0, (size_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp * sizeof(float)));
-		CU(cudaMalloc(&c->d_mag2[i], (size_t)c->max_dec * c->n_chp * sizeof(float)));
-	}
-	CU(cudaMalloc(&c->d_k1, (size_t)K1_NFIELDS * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_k2, (size_t)K2_NFIELDS * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_counters, (size_t)VDL2_NUM_COUNTERS * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_ring, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
-	CU(cudaMalloc(&c->d_free, (size_t)c->n_slots * 4));
-	CU(cudaMalloc(&c->d_ready, (size_t)c->n_slots * 4));
-	CU(cudaMalloc(&c->d_ctl, sizeof(vdl2_queue_ctl)));
 	CU(cudaMalloc(&c->d_events, (size_t)c->event_cap * sizeof(vdl2gpu_event)));
-	CU(cudaMemset(c->d_counters, 0, (size_t)VDL2_NUM_COUNTERS * c->n_chp * 4));
-	CU(cudaMemset(c->d_ring, 0, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
-	CU(cudaMemset(c->d_pool, 0, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
 
 	std::vector<uint32_t> k1, k2, centres, rates;
 	if(c->receivers) {
-		/* every channel mixes against its own receiver's centre (src/demod.c:385); the slot -> receiver tables K1 stages by */
-		std::vector<uint32_t> rx_first(n_rx + 1, 0);
+		/* every channel mixes against its own receiver's centre (src/demod.c:385) */
 		for(uint32_t r = 0; r < n_rx; r++) {
-			rx_first[r + 1] = rx_first[r] + rx[r].n_channels;
 			centres.insert(centres.end(), rx[r].n_channels, rx[r].centerfreq);
 			if(c->mixed) rates.insert(rates.end(), rx[r].n_channels, (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * rx_ex[r].oversample);
-		}
-		const uint32_t n_blocks = (c->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
-		std::vector<uint32_t> slot_rx((size_t)n_blocks * VDL2_RX_K1_BLOCK), block_rx(2 * (size_t)n_blocks);
-		c->rx_max = vdl2_rx_layout(n_blocks, c->lanes, c->full_warps, c->n_ch, rx_first.data(), n_rx, slot_rx.data(), block_rx.data());
-		c->rx_tile = c->mixed ? vdl2_rx_mixed_tile_groups(c->rx_max, c->rx_os_max) : vdl2_rx_tile_samples(c->rx_max, cfg->oversample);
-		CU(cudaMalloc(&c->d_slot_rx, slot_rx.size() * 4));
-		CU(cudaMalloc(&c->d_block_rx, block_rx.size() * 4));
-		CU(cudaMemcpy(c->d_slot_rx, slot_rx.data(), slot_rx.size() * 4, cudaMemcpyHostToDevice));
-		CU(cudaMemcpy(c->d_block_rx, block_rx.data(), block_rx.size() * 4, cudaMemcpyHostToDevice));
-		if(c->mixed) {
-			/* per receiver: oversample, format, place in a span; per slot: rate class; per class: the filter taps of
-			 * input_lpf_init(105000 x os) (src/demod.c:367-370) */
-			std::vector<uint32_t> os(n_rx), fmt(n_rx);
-			for(uint32_t r = 0; r < n_rx; r++) { os[r] = rx_ex[r].oversample; fmt[r] = rx_ex[r].sample_fmt; }
-			c->rx_in.resize(n_rx);
-			c->span_bytes_per_dec = vdl2_rx_span_layout(os.data(), fmt.data(), n_rx, c->rx_in.data());
-			for(uint32_t r = 0; r < n_rx; r++) {
-				c->span_pairs_per_dec += os[r];
-				c->cls_mask |= 1u << vdl2_rx_class(os[r]);
-			}
-			static const uint32_t class_os[3] = { 10, 13, 20 };
-			for(int k = 0; k < 3; k++) {
-				float A[3], B[3];
-				make_lpf((uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * class_os[k], A, B);
-				c->cls_taps[k][0] = A[0]; c->cls_taps[k][1] = A[1]; c->cls_taps[k][2] = A[2]; c->cls_taps[k][3] = B[1]; c->cls_taps[k][4] = B[2];
-			}
-			std::vector<uint8_t> slot_cls(slot_rx.size());
-			for(size_t s = 0; s < slot_rx.size(); s++) slot_cls[s] = (uint8_t)vdl2_rx_class(os[slot_rx[s]]);
-			CU(cudaMalloc(&c->d_rx_in, c->rx_in.size() * sizeof(vdl2_rx_input)));
-			CU(cudaMalloc(&c->d_slot_cls, slot_cls.size()));
-			CU(cudaMemcpy(c->d_rx_in, c->rx_in.data(), c->rx_in.size() * sizeof(vdl2_rx_input), cudaMemcpyHostToDevice));
-			CU(cudaMemcpy(c->d_slot_cls, slot_cls.data(), slot_cls.size(), cudaMemcpyHostToDevice));
-		}
-		if(c->ragged) {
-			c->rx_pos.assign(n_rx, 0);
-			c->rx_prev.assign(n_rx, 0);
-			c->ch_rx.resize(c->n_ch);
-			for(uint32_t r = 0; r < n_rx; r++) std::fill(c->ch_rx.begin() + rx_first[r], c->ch_rx.begin() + rx_first[r + 1], r);
-			c->rx_first = rx_first;
-			c->rx_centre.resize(n_rx);
-			for(uint32_t r = 0; r < n_rx; r++) c->rx_centre[r] = rx[r].centerfreq;
-			c->rx_restart_pending.assign(n_rx, 0);
 		}
 	}
 	initial_state(c->cfg, c->freqs.data(), c->receivers ? centres.data() : nullptr, c->mixed ? rates.data() : nullptr, c->n_ch, c->n_chp,
@@ -456,25 +527,6 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	memset(&ctl, 0, sizeof(ctl));
 	ctl.free_top = (int32_t)c->n_slots;
 	CU(cudaMemcpy(c->d_ctl, &ctl, sizeof(ctl), cudaMemcpyHostToDevice));
-
-	c->chunks.resize(n_inflight);
-	for(auto &s : c->chunks) {
-		/* h_raw / d_raw (max_chunk_bytes x n_streams each) are allocated by the first vdl2gpu_submit: hosts that only
-		 * use vdl2gpu_submit_device never need them */
-		CU(cudaHostAlloc((void **)&s.h_args, sizeof(vdl2_chunk_args), cudaHostAllocDefault));
-		CU(cudaMalloc(&s.d_args, sizeof(vdl2_chunk_args)));
-		if(c->ragged) {
-			CU(cudaHostAlloc((void **)&s.h_span, (size_t)n_rx * sizeof(vdl2_rx_span), cudaHostAllocDefault));
-			CU(cudaMalloc(&s.d_span, (size_t)n_rx * sizeof(vdl2_rx_span)));
-			CU(cudaHostAlloc((void **)&s.h_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart), cudaHostAllocDefault));
-			CU(cudaMalloc(&s.d_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart)));
-		}
-		CU(cudaHostAlloc((void **)&s.h_out, sizeof(vdl2_out_header) + c->out_cap, cudaHostAllocMapped));
-		CU(cudaHostGetDevicePointer((void **)&s.d_out, s.h_out, 0));
-		memset(s.h_out, 0, sizeof(vdl2_out_header));
-		CU(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-		for(auto &ev : s.tk) CU(cudaEventCreate(&ev));
-	}
 	return VDL2GPU_OK;
 }
 
@@ -532,6 +584,29 @@ extern "C" int vdl2gpu_create_receivers(const vdl2gpu_config *cfg, const vdl2gpu
 	return VDL2GPU_OK;
 }
 
+/* the checks of a mixed receiver list shared by vdl2gpu_create_mixed_receivers and vdl2gpu_update_receivers: the list's
+ * length, then every receiver (the reason goes to buf; *sum = the channels of the list) */
+static const char *mixed_count_error(const vdl2gpu_receiver_ex *rx, uint32_t n_rx) {
+	if(!rx || n_rx == 0) return "no receivers";
+	if(n_rx > 65535u) return "more than 65535 receivers (one K0 grid row each)";
+	return nullptr;
+}
+
+static const char *mixed_list_error(const vdl2gpu_receiver_ex *rx, uint32_t n_rx, char *buf, size_t cap, uint64_t *sum) {
+	*sum = 0;
+	for(uint32_t r = 0; r < n_rx; r++) {
+		if(rx[r].n_channels == 0) { snprintf(buf, cap, "receiver %u has no channels", r); return buf; }
+		if(rx[r].oversample != 10 && rx[r].oversample != 13 && rx[r].oversample != 20) {
+			snprintf(buf, cap, "receiver %u: oversample %u (10, 13 or 20 only)", r, rx[r].oversample); return buf;
+		}
+		if(rx[r].sample_fmt > 1) {
+			snprintf(buf, cap, "receiver %u: sample format %u (VDL2GPU_FMT_U8 or VDL2GPU_FMT_S16_LE only)", r, rx[r].sample_fmt); return buf;
+		}
+		*sum += rx[r].n_channels;
+	}
+	return nullptr;
+}
+
 extern "C" int vdl2gpu_create_mixed_receivers(const vdl2gpu_config *cfg, const vdl2gpu_receiver_ex *rx, uint32_t n_rx, vdl2gpu_ctx **out) {
 	const char *why = nullptr;
 	char buf[160];
@@ -539,20 +614,11 @@ extern "C" int vdl2gpu_create_mixed_receivers(const vdl2gpu_config *cfg, const v
 	if(!cfg || !out || !cfg->freqs || cfg->n_channels == 0) why = "bad vdl2gpu_config (no channels)";
 	else if(cfg->sample_rate || cfg->oversample || cfg->sample_fmt || cfg->centerfreq)
 		why = "cfg->sample_rate, oversample, sample_fmt and centerfreq must be 0 (they are per receiver)";
-	else if(!rx || n_rx == 0) why = "no receivers";
-	else if(n_rx > 65535u) why = "more than 65535 receivers (one K0 grid row each)";
+	else if((why = mixed_count_error(rx, n_rx))) {}
 	else if(cfg->n_streams != 0 && cfg->n_streams != n_rx) why = "n_streams must be 0 or the number of receivers";
 	else if(cfg->flags & VDL2GPU_FLAG_K1_SCALAR) why = "VDL2GPU_FLAG_K1_SCALAR is not available with receivers";
 	else {
-		for(uint32_t r = 0; r < n_rx && !why; r++) {
-			if(rx[r].n_channels == 0) { snprintf(buf, sizeof(buf), "receiver %u has no channels", r); why = buf; }
-			else if(rx[r].oversample != 10 && rx[r].oversample != 13 && rx[r].oversample != 20) {
-				snprintf(buf, sizeof(buf), "receiver %u: oversample %u (10, 13 or 20 only)", r, rx[r].oversample); why = buf;
-			} else if(rx[r].sample_fmt > 1) {
-				snprintf(buf, sizeof(buf), "receiver %u: sample format %u (VDL2GPU_FMT_U8 or VDL2GPU_FMT_S16_LE only)", r, rx[r].sample_fmt); why = buf;
-			}
-			sum += rx[r].n_channels;
-		}
+		why = mixed_list_error(rx, n_rx, buf, sizeof(buf), &sum);
 		if(!why && sum != cfg->n_channels) why = "the receivers' channel counts do not add up to n_channels";
 	}
 	if(why) {
@@ -1156,6 +1222,140 @@ extern "C" int vdl2gpu_restart_receiver(vdl2gpu_ctx *c, uint32_t r, uint32_t cen
 	if(freqs) std::copy(freqs, freqs + (c->rx_first[r + 1] - c->rx_first[r]), c->freqs.begin() + c->rx_first[r]);
 	if(!c->rx_restart_pending[r]) { c->rx_restart_pending[r] = 1; c->n_restart_pending++; }
 	return VDL2GPU_OK;
+}
+
+/* device memory freed on every way out of vdl2gpu_update_receivers */
+struct dev_scratch {
+	void *p = nullptr;
+	~dev_scratch() { cudaFree(p); }
+};
+
+/* vdl2gpu_update_receivers once everything is checked: the new layout n (setup_layout) is filled from the old one in c.
+ * Only n's buffers are written; c's are read. */
+static int migrate_receivers(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const vdl2gpu_receiver_ex *rx, const int32_t *from) {
+	const uint32_t n_rx = n->n_streams;
+	CU(cudaStreamSynchronize(c->stream));
+	CU(cudaStreamSynchronize(c->s_back));
+	vdl2_queue_ctl ctl;
+	CU(cudaMemcpy(&ctl, c->d_ctl, sizeof(ctl), cudaMemcpyDeviceToHost));
+	if(ctl.n_ready != 0) {           /* K3 empties the ready list of every span it decodes */
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_update_receivers: %u bursts wait in the ready list of a drained context", ctl.n_ready);
+		return VDL2GPU_EINVAL;
+	}
+	std::vector<uint32_t> old_slot_of_burst(c->n_chp);          /* K2_SLOT of every old slot: the pool slot its burst in progress holds */
+	CU(cudaMemcpy(old_slot_of_burst.data(), c->d_k2 + (size_t)K2_SLOT * c->n_chp, c->n_chp * 4, cudaMemcpyDeviceToHost));
+	std::vector<vdl2_rx_migrate> map(n->n_chp);
+	std::vector<uint8_t> held(n->n_slots, 0);
+	for(uint32_t i = 0; i < n->n_chp; i++) {
+		vdl2_rx_migrate &m = map[i];
+		memset(&m, 0, sizeof(m));
+		m.slot_from = vdl2_rx_slot_from(i, n->lanes, n->full_warps, n->n_ch, n->rx_first.data(), n_rx, from, c->lanes, c->full_warps,
+				c->rx_first.data());
+		m.chan_from = i < n->n_ch ? vdl2_rx_chan_from(i, n->rx_first.data(), n_rx, from, c->rx_first.data()) : -1;
+		uint32_t chan;
+		if(!vdl2_slot_channel(i, n->lanes, n->full_warps, n->n_ch, chan)) continue;
+		const uint32_t r = n->ch_rx[chan];
+		if(m.slot_from >= 0) {
+			m.hist_row = c->rx_prev[from[r]];
+			const int32_t b = (int32_t)old_slot_of_burst[m.slot_from];
+			if(b >= 0) held[b] = 1;                               /* (b < old n_slots <= n_slots: the index stays valid) */
+		} else {
+			m.dphi = vdl2_nco_dphi(rx[r].centerfreq, n->freqs[chan], (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * rx[r].oversample);
+			m.freq = n->freqs[chan];
+		}
+	}
+	/* the free list: every pool slot no kept channel holds (those of removed receivers come back) */
+	std::vector<int32_t> fl;
+	fl.reserve(n->n_slots);
+	for(uint32_t i = 0; i < n->n_slots; i++) if(!held[i]) fl.push_back((int32_t)i);
+	ctl.free_top = (int32_t)fl.size();
+	dev_scratch d_map;
+	CU(cudaMalloc(&d_map.p, map.size() * sizeof(vdl2_rx_migrate)));
+	CU(cudaMemcpy(d_map.p, map.data(), map.size() * sizeof(vdl2_rx_migrate), cudaMemcpyHostToDevice));
+	/* the plane the next span takes its history from: the other one of its own (run_chain) */
+	const int pb_prev = (int)((c->chunk_seq & 1u) ^ 1u);
+	vdl2_migrate_params p;
+	p.map = static_cast<const vdl2_rx_migrate *>(d_map.p);
+	p.n_chp = n->n_chp; p.old_n_chp = c->n_chp;
+	p.old_k1 = c->d_k1; p.old_k2 = c->d_k2; p.old_counters = c->d_counters; p.old_ring = c->d_ring; p.old_phase = c->d_phase2[pb_prev];
+	p.k1 = n->d_k1; p.k2 = n->d_k2; p.counters = n->d_counters; p.ring = n->d_ring; p.phase = n->d_phase2[pb_prev];
+	KL(vdl2_launch_migrate(&p, c->stream));
+	/* held slots keep their indices (and their words): K2 writes a burst's channel number into its slot only at hand-off */
+	CU(cudaMemcpyAsync(n->d_pool, c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot), cudaMemcpyDeviceToDevice, c->stream));
+	CU(cudaMemcpyAsync(n->d_free, fl.data(), fl.size() * 4, cudaMemcpyHostToDevice, c->stream));
+	CU(cudaMemcpyAsync(n->d_ctl, &ctl, sizeof(ctl), cudaMemcpyHostToDevice, c->stream));
+	CU(cudaStreamSynchronize(c->stream));
+	/* per receiver: a kept one carries its position and a pending restart over; every history now starts at row 0 */
+	for(uint32_t r = 0; r < n_rx; r++) {
+		if(from[r] < 0) continue;
+		n->rx_pos[r] = c->rx_pos[from[r]];
+		n->rx_restart_pending[r] = c->rx_restart_pending[from[r]];
+		n->n_restart_pending += n->rx_restart_pending[r];
+	}
+	return VDL2GPU_OK;
+}
+
+/* Replace the receiver list of a drained ragged context (see include/vdl2gpu.h).  Everything is checked first; then the
+ * new layout is allocated beside the old one, the kept channels' state is moved into it, the context switches to it and
+ * the old one is freed.  Any failure before the switch frees the new layout and leaves the context as it was. */
+extern "C" int vdl2gpu_update_receivers(vdl2gpu_ctx *c, const vdl2gpu_receiver_ex *rx, const int32_t *from, uint32_t n_rx,
+		const uint32_t *freqs) {
+	const char *why = nullptr;
+	char buf[192];
+	uint64_t sum = 0;
+	if(!c) why = "no context";
+	else if(!c->ragged) why = "needs a context made by vdl2gpu_create_mixed_receivers with VDL2GPU_FLAG_RAGGED";
+	else if(vdl2gpu_chunks_in_flight(c) != 0) why = "spans are in flight (vdl2gpu_flush first)";
+	else if((why = mixed_count_error(rx, n_rx))) {}
+	else if(!from || !freqs) why = "from and freqs must not be NULL";
+	else if((why = mixed_list_error(rx, n_rx, buf, sizeof(buf), &sum))) {}
+	else {
+		std::vector<uint8_t> seen(c->n_streams, 0);
+		uint64_t first = 0;
+		for(uint32_t r = 0; r < n_rx && !why; first += rx[r].n_channels, r++) {
+			if(from[r] == -1) continue;
+			const uint32_t o = (uint32_t)from[r];
+			if(from[r] < -1 || o >= c->n_streams) { snprintf(buf, sizeof(buf), "entry %u continues receiver %d of %u", r, from[r], c->n_streams); why = buf; }
+			else if(seen[o]) { snprintf(buf, sizeof(buf), "entry %u continues receiver %u, which an earlier entry continues", r, o); why = buf; }
+			else if(rx[r].centerfreq != c->rx_centre[o] || rx[r].n_channels != c->rx_first[o + 1] - c->rx_first[o]
+					|| rx[r].oversample != c->rx_in[o].oversample || rx[r].sample_fmt != c->rx_in[o].fmt
+					|| !std::equal(freqs + first, freqs + first + rx[r].n_channels, c->freqs.begin() + c->rx_first[o])) {
+				snprintf(buf, sizeof(buf), "entry %u does not repeat receiver %u's centre, channels, oversample, format and frequencies "
+						"(retune with vdl2gpu_restart_receiver)", r, o);
+				why = buf;
+			}
+			if(!why) seen[o] = 1;
+		}
+		if(!why && sum > 0xFFFFFFFFull) why = "more than 2^32 - 1 channels";
+	}
+	if(why) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_update_receivers: %s", why);
+		return VDL2GPU_EINVAL;
+	}
+	CU(cudaSetDevice(c->device));
+	vdl2gpu_config cfg = c->cfg;
+	cfg.n_channels = (uint32_t)sum;
+	cfg.freqs = freqs;
+	cfg.n_streams = n_rx;
+	std::vector<vdl2gpu_receiver> base(n_rx);
+	for(uint32_t r = 0; r < n_rx; r++) { base[r].centerfreq = rx[r].centerfreq; base[r].n_channels = rx[r].n_channels; }
+	vdl2gpu_ctx *n = new vdl2gpu_ctx();
+	n->cfg = c->cfg;
+	n->device = c->device; n->n_sms = c->n_sms;
+	n->receivers = n->mixed = n->ragged = true;
+	n->n_streams = n_rx;
+	n->cfg.n_streams = n_rx;
+	int rc = setup_layout(n, &cfg, base.data(), n_rx, rx, c->n_slots, "vdl2gpu_update_receivers");
+	if(rc == VDL2GPU_OK) rc = migrate_receivers(c, n, rx, from);
+	if(rc == VDL2GPU_OK) {
+		swap_layout(c, n);
+		/* the graphs went with the old chunk slots: the next spans capture anew, as after create */
+		c->graph_nominal = 0;
+		c->last_n_dec = 0;
+	}
+	free_layout(n);
+	delete n;
+	return rc;
 }
 
 extern "C" int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *c, uint64_t *out, uint32_t n_rx) {

@@ -1671,3 +1671,42 @@ extern "C" int vdl2_launch_rs(uint8_t *blocks, const int32_t *fec_octets, uint32
 	k_rs_verify<<<(n + 63) / 64, 64, 0, st>>>(blocks, fec_octets, n, ret, tables);
 	return (int)cudaGetLastError();
 }
+
+/* ------------------------------------------------------------------------------------------------
+ * Receivers joining and leaving a ragged context (vdl2gpu_update_receivers): one thread per slot of the new planes gathers
+ * its channel's state from the old planes (vdl2_rx_migrate), or writes the fresh state create writes.  A kept slot takes
+ * its K1 and K2 fields, its syncbuf ring and its last 160 phases: rows [hist_row, hist_row + 160) of the old plane the next
+ * span would have taken its history from become rows [0, 160) of the new one, which the host then pairs with prev_n = 0.
+ * Thread i also fills channel i of the per-channel counters, which are kept by channel.
+ * ---------------------------------------------------------------------------------------------- */
+__global__ void __launch_bounds__(256) k_migrate_receivers(vdl2_migrate_params p) {
+	const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+	if(i >= p.n_chp) return;
+	const vdl2_rx_migrate m = p.map[i];
+	const size_t s = p.n_chp, so = p.old_n_chp;
+	if(m.slot_from >= 0) {
+		const size_t o = (size_t)m.slot_from;
+		for(int f = 0; f < K1_NFIELDS; f++) p.k1[f * s + i] = p.old_k1[f * so + o];
+		for(int f = 0; f < K2_NFIELDS; f++) p.k2[f * s + i] = p.old_k2[f * so + o];
+		for(uint32_t t = 0; t < VDL2_SYNC_BUFLEN; t++) {
+			p.ring[t * s + i] = p.old_ring[t * so + o];
+			p.phase[t * s + i] = p.old_phase[(m.hist_row + t) * so + o];
+		}
+	} else {
+		for(int f = 0; f < K1_NFIELDS; f++) p.k1[f * s + i] = 0u;
+		for(int f = 0; f < K2_NFIELDS; f++) p.k2[f * s + i] = 0u;
+		if(m.slot_from == VDL2_MIGRATE_FRESH) {
+			vdl2_k1_fresh(p.k1, s, i, m.dphi);
+			vdl2_chan v;
+			vdl2_chan_init(v, m.freq);
+			vdl2_chan_store(v, p.k2, s, i);
+		}
+		for(uint32_t t = 0; t < VDL2_SYNC_BUFLEN; t++) { p.ring[t * s + i] = 0.f; p.phase[t * s + i] = 0.f; }
+	}
+	for(int k = 0; k < VDL2_NUM_COUNTERS; k++) p.counters[k * s + i] = m.chan_from >= 0 ? p.old_counters[k * so + (size_t)m.chan_from] : 0u;
+}
+
+extern "C" int vdl2_launch_migrate(const vdl2_migrate_params *p, cudaStream_t st) {
+	k_migrate_receivers<<<(p->n_chp + 255u) / 256u, 256, 0, st>>>(*p);
+	return (int)cudaGetLastError();
+}

@@ -137,6 +137,18 @@ typedef struct {
 	uint32_t abandoned;          /* the ready list may hold slots given up by a restart (VDL2_READY_ABANDONED) */
 } vdl2_k3_params;
 
+/* receivers joining and leaving (k_migrate_receivers): the new per-channel planes (stride n_chp) from the old ones (stride
+ * old_n_chp), entry i of `map` for slot i and channel i */
+typedef struct {
+	const vdl2_rx_migrate *map;  /* [n_chp] */
+	uint32_t n_chp, old_n_chp;
+	const uint32_t *old_k1, *old_k2, *old_counters;
+	const float *old_ring;
+	const float *old_phase;      /* the old plane the next span would have taken its history rows from */
+	uint32_t *k1, *k2, *counters;
+	float *ring, *phase;         /* phase: the new plane the next span takes its history rows from */
+} vdl2_migrate_params;
+
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -164,6 +176,7 @@ int vdl2_launch_k2(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k3(const vdl2_k3_params *p, uint32_t grid, cudaStream_t st);
 int vdl2_launch_k4(const uint8_t *frames, const uint32_t *offsets, const uint32_t *lens, uint32_t n, uint16_t *out, cudaStream_t st);
 int vdl2_launch_rs(uint8_t *blocks, const int32_t *fec_octets, uint32_t n, int32_t *ret, const vdl2_tables *tables, cudaStream_t st);
+int vdl2_launch_migrate(const vdl2_migrate_params *p, cudaStream_t st);
 #ifdef __cplusplus
 }
 #endif

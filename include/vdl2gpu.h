@@ -228,6 +228,32 @@ int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *ctx, uint64_t *out, uint32_t n_r
  * Returns VDL2GPU_EINVAL, before the device is touched, for a NULL context, r >= n_rx, or any context but a ragged
  * mixed-receivers one. */
 int vdl2gpu_restart_receiver(vdl2gpu_ctx *ctx, uint32_t r, uint32_t centerfreq, const uint32_t *freqs);
+/* Replace the receivers of a drained ragged mixed-receivers context (VDL2GPU_FLAG_RAGGED) with rx[0..n_rx): receivers
+ * join, leave, move within the list, or are swapped for a device of another kind (remove it and add the new one), and
+ * every other receiver carries on as if nothing had happened.  freqs lists the channels receiver by receiver, as for
+ * vdl2gpu_create_mixed_receivers.
+ *   - from[i] >= 0: entry i continues old receiver from[i] and repeats its current description (centre, channel count,
+ *     oversample, format and channel frequencies, after any restarts; a retune is vdl2gpu_restart_receiver's job).  Each
+ *     old receiver appears at most once; those not listed are removed.
+ *   - from[i] == -1: a new receiver, which decodes what a freshly started reference process decodes from what it brings:
+ *     position 0, burst_seq 0, zero counters.
+ *   - A kept receiver keeps its demodulator state, its burst in progress (delivered later under its new channel numbers),
+ *     its position (vdl2gpu_get_receiver_positions), sync_dec_index, timestamps, burst_seq and counters, and a restart
+ *     still pending applies with the next span.  A removed receiver's burst in progress is dropped without a frame, a trace
+ *     event or a counter change, and its counters are gone (read them first).
+ *   - Only on a drained context (vdl2gpu_chunks_in_flight == 0, as after vdl2gpu_flush): frames delivered before the call
+ *     carry the old channel numbers and frames delivered after it the new ones.  Trace events not yet read still carry the
+ *     old numbers.  vdl2gpu_read_dec has no rows until a span runs.  max_span follows the create rule for the new list: a
+ *     receiver with more bytes per decimated sample than any before shortens the longest allowed span.
+ *   - The context is rebuilt: the new buffers are allocated before the old ones are freed, so the device briefly holds both
+ *     (about 2 x 9 GB for 2048 receivers x 8 channels at the default max_chunk_bytes), and the next spans recapture their
+ *     CUDA graphs.
+ * Returns VDL2GPU_EINVAL for a NULL context, any context but a ragged mixed-receivers one, spans in flight, a bad from[]
+ * (out of range, repeated, or a changed description), and the receiver checks of vdl2gpu_create_mixed_receivers (none,
+ * more than 65535, oversample, format, no channels); VDL2GPU_ETOOBIG past the kernels' 32-bit element index.  Refusals
+ * touch neither the context nor the device; a CUDA or allocation failure during the rebuild leaves the context as it was. */
+int vdl2gpu_update_receivers(vdl2gpu_ctx *ctx, const vdl2gpu_receiver_ex *rx, const int32_t *from, uint32_t n_rx,
+		const uint32_t *freqs);
 int vdl2gpu_wait_input_consumed(vdl2gpu_ctx *ctx, void *stream);
 /* Make `stream` (cudaStream_t) wait for all device work enqueued by this context so far (for timing with
  * events recorded on the caller's stream, and for ordering consumers of device-side results). */
