@@ -93,6 +93,8 @@ def load_library():
     L.vdl2gpu_get_receiver_positions.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_restart_receiver.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
     L.vdl2gpu_update_receivers.argtypes = [C.c_void_p, C.POINTER(_ReceiverEx), C.c_void_p, C.c_uint32, C.c_void_p]
+    L.vdl2gpu_push.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+    L.vdl2gpu_submit_pushed.argtypes = [C.c_void_p]
     L.vdl2gpu_destroy.argtypes = [C.c_void_p]
     L.vdl2gpu_submit.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_submit_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
@@ -420,7 +422,9 @@ class Vdl2MixedReceivers(Vdl2Receivers):
 
     With ragged=True the receivers do not advance in lock step: submit_ragged() takes whatever whole decimation groups each
     receiver has (any count, 0 included, per receiver and per span), and every receiver still decodes exactly what one
-    reference process decodes from the concatenation of its buffers.  restart_receiver() starts one receiver afresh (a
+    reference process decodes from the concatenation of its buffers.  push() queues any length of one receiver's bytes
+    inside the library (one call per device callback, from that device's own thread) and submit_pushed() turns what is
+    queued into spans.  restart_receiver() starts one receiver afresh (a
     reconnect, a swapped device, a retune) without disturbing the others, and update_receivers() / add_receivers() /
     remove_receivers() let receivers join and leave (after flush()) while the others carry on."""
 
@@ -523,6 +527,20 @@ class Vdl2MixedReceivers(Vdl2Receivers):
             raise ValueError(f"{n.size} counts for {self.n_receivers} receivers")
         _check(self.L, self.L.vdl2gpu_submit_ragged_device(self.h, C.c_void_p(dev_ptr), n.ctypes.data, C.c_void_p(producer_stream)),
                "vdl2gpu_submit_ragged_device")
+
+    def push(self, r, buf):
+        """queue receiver r's next bytes (any length up to max_chunk_bytes, in its own format; may split a decimation group
+        or a sample); blocks while the receiver's ring lacks room.  The GIL is released during the call, so one Python
+        thread per receiver pushes concurrently."""
+        b = np.ascontiguousarray(buf).view(np.uint8).reshape(-1)
+        if b.size > 0xFFFFFFFF:                      # the C length is 32 bits: refuse rather than push size mod 2^32
+            raise Vdl2GpuError(f"vdl2gpu_push: {b.size} bytes, more than max_chunk_bytes")
+        _check(self.L, self.L.vdl2gpu_push(self.h, int(r), b.ctypes.data if b.size else None, b.size), "vdl2gpu_push")
+
+    def submit_pushed(self):
+        """submit spans of the whole decimation groups queued when the call starts (bytes pushed during the call wait for the
+        next one); returns the number of spans"""
+        return _check(self.L, self.L.vdl2gpu_submit_pushed(self.h), "vdl2gpu_submit_pushed")
 
     def receiver_positions(self):
         """decimated samples accepted so far per receiver (uint64[n_receivers])"""

@@ -1396,4 +1396,92 @@ typedef struct {
 	int32_t chan_from;           /* channel i: the old channel whose counters it continues, or -1 (zero counters) */
 } vdl2_rx_migrate;
 
+/* ------------------------------------------------------------------------------------------------
+ * Pushed input (vdl2gpu_push / vdl2gpu_submit_pushed on a ragged context): every receiver has a byte ring in device memory
+ * (mirrored byte for byte in pinned host memory) that its pushes fill at any length and spans drain in whole decimation
+ * groups.  Positions are 64-bit stream positions, bytes pushed since the ring was made; a position's place in the ring is
+ * position mod cap.  Per receiver: head (bytes pushed), tail (first byte not yet taken into a span or dropped) and freed
+ * (every byte before it has been read by the copies and the K0 that needed it, so it may be overwritten).
+ * ---------------------------------------------------------------------------------------------- */
+/* receiver r's ring: bytes [base, base + cap) of the ring buffer */
+typedef struct {
+	uint64_t base, cap;
+} vdl2_rx_ring;
+
+/* Ring capacity of a receiver of group_bytes (oversample x bytes per complex sample) bytes per decimated sample: one push
+ * of max_chunk_bytes, a full span of max_span groups and one group (a remainder that waits for the next push), rounded up
+ * to 16 bytes.  A multiple of the sample size (2 or 4) and every span fits, so no sample straddles the end of the ring. */
+VDL2_HD uint64_t vdl2_push_ring_cap(uint32_t max_chunk_bytes, uint32_t max_span, uint32_t group_bytes) {
+	const uint64_t need = (uint64_t)max_chunk_bytes + ((uint64_t)max_span + 1u) * group_bytes;
+	return (need + 15u) & ~(uint64_t)15u;
+}
+
+/* the rings of all receivers back to back, each 16-byte aligned; returns the bytes of the ring buffer */
+VDL2_HD uint64_t vdl2_push_ring_layout(const vdl2_rx_input *rx, uint32_t n_rx, uint32_t max_chunk_bytes, uint32_t max_span, vdl2_rx_ring *out) {
+	uint64_t base = 0;
+	for(uint32_t r = 0; r < n_rx; r++) {
+		out[r].base = base;
+		out[r].cap = vdl2_push_ring_cap(max_chunk_bytes, max_span, rx[r].oversample * (rx[r].fmt == 1u ? 4u : 2u));
+		base += out[r].cap;
+	}
+	return base;
+}
+
+/* bytes a push may write without touching a byte still queued or in flight */
+VDL2_HD uint64_t vdl2_push_room(uint64_t cap, uint64_t head, uint64_t freed) { return cap - (head - freed); }
+
+/* the one or two pieces of `len` bytes at stream position pos in a ring of cap bytes: ring offsets off[k], lengths len[k]
+ * (len[1] = 0 unless the bytes wrap) */
+typedef struct {
+	uint64_t off[2];
+	uint64_t len[2];
+} vdl2_ring_segs;
+
+VDL2_HD vdl2_ring_segs vdl2_ring_segments(uint64_t cap, uint64_t pos, uint64_t len) {
+	vdl2_ring_segs s;
+	s.off[0] = pos % cap;
+	s.len[0] = len < cap - s.off[0] ? len : cap - s.off[0];
+	s.off[1] = 0;
+	s.len[1] = len - s.len[0];
+	return s;
+}
+
+/* a span's take from one receiver: its whole queued groups, at most max_span */
+VDL2_HD uint32_t vdl2_push_take(uint64_t head, uint64_t tail, uint32_t group_bytes, uint32_t max_span) {
+	const uint64_t g = (head - tail) / group_bytes;
+	return g < max_span ? (uint32_t)g : max_span;
+}
+
+/* the write position after a restart drops the queue: the next sample boundary at or after head (the queue's bytes,
+ * a split sample included, belong to the old process) */
+VDL2_HD uint64_t vdl2_push_realign(uint64_t head, uint32_t bpp) { return (head + bpp - 1u) / bpp * bpp; }
+
+/* The table of one pushed span: as vdl2_rx_span_table, but receiver r's off is the ring offset of its tail (the span's
+ * first byte) and its tail advances by n[r] groups */
+VDL2_HD void vdl2_push_span_table(const vdl2_rx_input *rx, const vdl2_rx_ring *ring, uint32_t n_rx, const uint32_t *n, uint64_t *tail,
+		uint64_t *pos, uint32_t *prev, vdl2_rx_span *out) {
+	for(uint32_t r = 0; r < n_rx; r++) {
+		out[r].off = tail[r] % ring[r].cap;
+		out[r].n = n[r];
+		out[r].prev_n = prev[r];
+		out[r].dec_base = pos[r];
+		tail[r] += (uint64_t)n[r] * rx[r].oversample * (rx[r].fmt == 1u ? 4u : 2u);
+		pos[r] += n[r];
+		prev[r] = n[r];
+	}
+}
+
+/* Timestamp anchor of a burst whose sync lies in decimation group `sync` of a receiver: the stream position just past
+ * the last input sample of that group, given a span that took groups from dec_base on starting at stream position
+ * byte_base */
+VDL2_HD uint64_t vdl2_push_sync_end(uint64_t sync, uint64_t dec_base, uint64_t byte_base, uint32_t group_bytes) {
+	return byte_base + (sync - dec_base + 1u) * group_bytes;
+}
+
+/* ... and how far before its push's arrival that sample arrived: the input samples the push (which ends at stream
+ * position push_end) carried after it, at the receiver's rate (samples per second) */
+VDL2_HD double vdl2_push_back_seconds(uint64_t sample_end, uint64_t push_end, uint32_t bpp, uint32_t rate) {
+	return (double)((push_end - sample_end) / bpp) / (double)rate;
+}
+
 #endif

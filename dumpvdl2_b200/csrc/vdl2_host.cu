@@ -15,7 +15,11 @@
 #include <string.h>
 #include <sys/time.h>
 #include <algorithm>
+#include <atomic>
+#include <condition_variable>
 #include <deque>
+#include <functional>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -64,11 +68,28 @@ struct chunk_slot {
 	 * path, so the graphs of ordinary spans never see the table */
 	vdl2_rx_restart *h_restart = nullptr, *d_restart = nullptr;
 	bool restart = false;
+	/* pushed spans (vdl2gpu_submit_pushed): K0 reads the receivers' rings; k0_done is recorded after it (ragged contexts) */
+	bool pushed = false;
+	cudaEvent_t k0_done = nullptr;
 	cudaGraphExec_t g_front[6] = { nullptr }, g_k2a[6] = { nullptr }, g_back[6] = { nullptr };    /* index = chunk number mod 6 (dec buffer, plane) */
 	uint32_t graph_pairs[6] = { 0 };
 	uint64_t first_pair = 0, dec_base = 0;
 	uint32_t n_pairs = 0, n_dec = 0;
 	struct timeval arrival = { 0, 0 };
+};
+
+/* Pushed input of one receiver (vdl2gpu_push).  Stream positions as in vdl2_core.cuh: head, tail, freed.  A fence says
+ * that once `ev` has completed, every byte before `pos` has been read by whatever copy or K0 needed it. */
+struct ring_fence { cudaEvent_t ev; uint64_t pos; };
+struct push_rec { uint64_t end; double t; };                /* a push: the stream position it ended at, its arrival time */
+struct span_anchor { uint64_t dec_base, byte_base; uint32_t n; };   /* a pushed span took groups [dec_base, + n) from byte_base on */
+struct push_rx {
+	std::mutex m;                                       /* head, tail, freed, fences, recs (pushes of this receiver and the control thread) */
+	std::condition_variable room;                       /* a push waiting for the control thread to take its queue into spans */
+	uint64_t head = 0, tail = 0, freed = 0;
+	std::deque<ring_fence> fences;
+	std::deque<push_rec> recs;
+	std::deque<span_anchor> anchors;                    /* (control thread only) */
 };
 
 struct vdl2gpu_ctx {
@@ -154,6 +175,17 @@ struct vdl2gpu_ctx {
 	std::vector<pending_frame> pending;
 	std::vector<std::vector<uint8_t>> blobs;
 	cudaEvent_t ev_drain = nullptr;
+	/* pushed input (ragged contexts, allocated by the first vdl2gpu_push): the receivers' rings (vdl2_push_ring_layout) in
+	 * device memory and their pinned host mirror, the copy stream every push issues its copies on, the event a restart
+	 * records there when it drops queued bytes, and per receiver its queue state */
+	std::mutex push_alloc;
+	std::atomic<bool> push_ready{false};
+	uint8_t *d_rings = nullptr, *h_rings = nullptr;
+	std::vector<vdl2_rx_ring> rings;
+	vdl2_rx_ring *d_ring_tab = nullptr;
+	cudaStream_t s_copy = nullptr;
+	cudaEvent_t ev_copied = nullptr, ev_dropped = nullptr;
+	std::vector<std::unique_ptr<push_rx>> push;
 };
 
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
@@ -191,6 +223,7 @@ static void free_layout(vdl2gpu_ctx *c) {
 		if(s.d_raw) cudaFree(s.d_raw);
 		if(s.h_out) cudaFreeHost(s.h_out);
 		if(s.done) cudaEventDestroy(s.done);
+		if(s.k0_done) cudaEventDestroy(s.k0_done);
 		for(auto &e : s.tk) if(e) cudaEventDestroy(e);
 		for(int i = 0; i < 6; i++) {
 			if(s.g_front[i]) cudaGraphExecDestroy(s.g_front[i]);
@@ -214,12 +247,27 @@ static void free_layout(vdl2gpu_ctx *c) {
 	cudaFree(c->d_rx_in); cudaFree(c->d_slot_cls);
 }
 
+/* the pushed-input rings and their queues (no push, copy or span may be running on them) */
+static void free_rings(vdl2gpu_ctx *c) {
+	if(c->s_copy) cudaStreamSynchronize(c->s_copy);
+	cudaFree(c->d_rings); cudaFree(c->d_ring_tab);
+	if(c->h_rings) cudaFreeHost(c->h_rings);
+	c->d_rings = c->h_rings = nullptr; c->d_ring_tab = nullptr;
+	c->rings.clear();
+	c->push.clear();
+	c->push_ready = false;
+}
+
 static int free_ctx(vdl2gpu_ctx *c) {
 	if(!c) return VDL2GPU_OK;
 	cudaSetDevice(c->device);
 	if(c->stream) cudaStreamSynchronize(c->stream);
 	if(c->s_mid) cudaStreamSynchronize(c->s_mid);
 	if(c->s_back) cudaStreamSynchronize(c->s_back);
+	free_rings(c);
+	if(c->ev_copied) cudaEventDestroy(c->ev_copied);
+	if(c->ev_dropped) cudaEventDestroy(c->ev_dropped);
+	if(c->s_copy) cudaStreamDestroy(c->s_copy);
 	free_layout(c);
 	cudaFree(c->d_tab); cudaFree(c->d_events); cudaFree(c->d_block_trace);
 	if(c->ev_input_ready) cudaEventDestroy(c->ev_input_ready);
@@ -389,6 +437,7 @@ static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu
 			CU(cudaMalloc(&s.d_span, (size_t)n_rx * sizeof(vdl2_rx_span)));
 			CU(cudaHostAlloc((void **)&s.h_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart), cudaHostAllocDefault));
 			CU(cudaMalloc(&s.d_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart)));
+			CU(cudaEventCreateWithFlags(&s.k0_done, cudaEventDisableTiming));
 		}
 		CU(cudaHostAlloc((void **)&s.h_out, sizeof(vdl2_out_header) + c->out_cap, cudaHostAllocMapped));
 		CU(cudaHostGetDevicePointer((void **)&s.d_out, s.h_out, 0));
@@ -648,9 +697,11 @@ static uint32_t synd_weight_of(uint32_t syn) {       /* src/decode.c:98-100 */
 /* burst records (region = vdl2_out_header + records) -> frames.  Offsets in the pending frames are relative to the
  * first record.  `dec_end` / `arrival` place the burst in time (see burst_timestamp below); with ragged spans `span` (the
  * span's receiver table) and `ch_rx` (channel -> receiver) give each channel its own receiver's end position instead. */
+typedef std::function<bool(uint32_t channel, uint64_t sync, double &ts)> stamp_fn;
+
 static void parse_region(const uint8_t *region, uint32_t out_cap, double rate, struct timeval arrival, uint64_t dec_end,
 		uint32_t blob_id, std::vector<pending_frame> &pending, vdl2gpu_stats &stats, const vdl2_rx_span *span = nullptr,
-		const uint32_t *ch_rx = nullptr) {
+		const uint32_t *ch_rx = nullptr, const stamp_fn *stamp = nullptr) {
 	vdl2_out_header h;
 	memcpy(&h, region, sizeof(h));
 	const uint8_t *base = region + sizeof(vdl2_out_header);
@@ -702,6 +753,8 @@ static void parse_region(const uint8_t *region, uint32_t out_cap, double rate, s
 			 * being processed when the burst completed, moved back by the distance to the sync sample */
 			double back = end > sync_idx ? ((double)end - (double)sync_idx) / rate : 0.0;
 			double ts = (double)arrival.tv_sec + 1e-6 * (double)arrival.tv_usec - back;
+			/* pushed spans: from the arrival of the push that carried the sync group (push_stamp) */
+			if(stamp) (*stamp)(r->channel, sync_idx, ts);
 			pf.f.burst_timestamp.tv_sec = (time_t)floor(ts);
 			pf.f.burst_timestamp.tv_usec = (suseconds_t)((ts - floor(ts)) * 1e6);
 			pf.f.fcs_residue = (uint16_t)crc;
@@ -711,6 +764,26 @@ static void parse_region(const uint8_t *region, uint32_t out_cap, double rate, s
 			pending.push_back(pf);
 		}
 	}
+}
+
+/* Timestamp of a burst of a pushed span whose sync lies in decimation group `sync` of channel chan's receiver: the
+ * arrival time of the push that carried the group's last input sample, moved back by the input samples that push carried
+ * after it.  False when the group was not taken from pushed bytes (the span-end rule of parse_region then stands). */
+static bool push_stamp(vdl2gpu_ctx *c, uint32_t chan, uint64_t sync, double &ts) {
+	const uint32_t r = c->ch_rx[chan];
+	push_rx &q = *c->push[r];
+	const vdl2_rx_input &in = c->rx_in[r];
+	const uint32_t bpp = in.fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
+	auto a = std::upper_bound(q.anchors.begin(), q.anchors.end(), sync, [](uint64_t v, const span_anchor &x) { return v < x.dec_base; });
+	if(a == q.anchors.begin()) return false;
+	--a;
+	if(sync >= a->dec_base + a->n) return false;
+	const uint64_t end = vdl2_push_sync_end(sync, a->dec_base, a->byte_base, in.oversample * bpp);
+	std::lock_guard<std::mutex> lk(q.m);
+	auto p = std::lower_bound(q.recs.begin(), q.recs.end(), end, [](const push_rec &x, uint64_t v) { return x.end < v; });
+	if(p == q.recs.end()) return false;
+	ts = p->t - vdl2_push_back_seconds(end, p->end, bpp, (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * in.oversample);
+	return true;
 }
 
 static void harvest(vdl2gpu_ctx *c, chunk_slot &s) {
@@ -738,8 +811,10 @@ static void harvest(vdl2gpu_ctx *c, chunk_slot &s) {
 	const uint32_t blob_id = (uint32_t)c->blobs.size() - 1;
 	/* decimated samples per second (105000 for every receiver of a mixed context, whose config carries no rate) */
 	const double rate = c->mixed ? (double)VDL2_SYMBOL_RATE * VDL2_SPS : (double)c->cfg.sample_rate / (double)c->cfg.oversample;
+	stamp_fn stamp;
+	if(s.pushed) stamp = [c](uint32_t chan, uint64_t sync, double &ts) { return push_stamp(c, chan, sync, ts); };
 	parse_region(c->blobs.back().data(), c->out_cap, rate, s.arrival, s.dec_base + s.n_dec, blob_id, c->pending, c->stats,
-			c->ragged ? s.h_span : nullptr, c->ch_rx.data());
+			c->ragged ? s.h_span : nullptr, c->ch_rx.data(), s.pushed ? &stamp : nullptr);
 	c->stats.chunks_completed++;
 	s.busy = false;
 }
@@ -790,6 +865,7 @@ static int acquire_slot(vdl2gpu_ctx *c, chunk_slot **out) {
 		harvest(c, s);
 		if(!c->inflight.empty() && c->inflight.front() == c->next_slot) c->inflight.pop_front();
 	}
+	s.pushed = false;
 	*out = &s;
 	return VDL2GPU_OK;
 }
@@ -860,6 +936,11 @@ static int launch_k0_mixed(vdl2gpu_ctx *c, const void *d_raw, uint32_t n_dec, co
 /* mixed-rate receivers: K0 of a span of n_dec decimated samples (ragged spans: n_dec is the width, the slot's table the counts) */
 static int launch_k0_span(vdl2gpu_ctx *c, const chunk_slot &s, const void *d_raw, uint32_t n_dec, const vdl2_chunk_args *ca) {
 	if(!c->ragged) return launch_k0_mixed(c, d_raw, n_dec, ca);
+	if(s.pushed) {                                      /* (never captured: pushed spans take the direct path) */
+		KL(vdl2_launch_k0_rings(c->d_rings, n_dec, c->d_rx_in, c->d_ring_tab, s.d_span, c->n_streams, c->rx_os_max, c->d_tab->levels,
+				reinterpret_cast<float *>(c->d_samples), c->max_pairs, c->stream));
+		return VDL2GPU_OK;
+	}
 	KL(vdl2_launch_k0_ragged(d_raw, n_dec, c->d_rx_in, s.d_span, c->n_streams, c->rx_os_max, c->d_tab->levels,
 			reinterpret_cast<float *>(c->d_samples), c->max_pairs, ca, c->stream));
 	return VDL2GPU_OK;
@@ -931,7 +1012,7 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
 	const bool overlap = c->s_back != c->stream;
 	s.seq = seq;
-	bool graph = c->use_graphs && !planar && overlap;
+	bool graph = c->use_graphs && !planar && overlap && !s.pushed;     /* pushed spans take the direct path */
 	if(graph && c->graph_nominal == 0) c->graph_nominal = n_pairs;
 	graph = graph && n_pairs == c->graph_nominal;            /* odd-sized chunks (the tail of a file) take the direct path */
 	graph = graph && !s.restart;                             /* ... and so do spans that restart receivers */
@@ -955,8 +1036,11 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	} else {
 		if(c->ragged) CU(cudaMemcpyAsync(s.d_span, s.h_span, c->n_streams * sizeof(vdl2_rx_span), cudaMemcpyHostToDevice, c->stream));
 		if(s.restart) CU(cudaMemcpyAsync(s.d_restart, s.h_restart, c->n_chp * sizeof(vdl2_rx_restart), cudaMemcpyHostToDevice, c->stream));
-		if(c->mixed) { int rc = launch_k0_span(c, s, d_raw, n_pairs, nullptr); if(rc) return rc; }
-		else if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
+		if(c->mixed) {
+			int rc = launch_k0_span(c, s, d_raw, n_pairs, nullptr);
+			if(rc) return rc;
+			if(s.pushed) CU(cudaEventRecord(s.k0_done, c->stream));     /* the rings' bytes of this span are read */
+		} else if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 				n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, nullptr, c->stream));
 		else KL(vdl2_launch_k0(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 				n_pairs * bpp, c->max_pairs, nullptr, c->stream));
@@ -1153,6 +1237,22 @@ static void fill_restarts(vdl2gpu_ctx *c, chunk_slot &s) {
 	c->n_restart_pending = 0;
 }
 
+/* bytes per decimation group of receiver r of a mixed context */
+static inline uint32_t group_bytes(const vdl2gpu_ctx *c, uint32_t r) {
+	return c->rx_in[r].oversample * (c->rx_in[r].fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
+}
+
+/* whether any receiver has pushed bytes not yet in a span (whole_group: at least one whole decimation group of them) */
+static bool push_queued(vdl2gpu_ctx *c, bool whole_group) {
+	if(!c->push_ready) return false;
+	for(uint32_t r = 0; r < c->n_streams; r++) {
+		push_rx &q = *c->push[r];
+		std::lock_guard<std::mutex> lk(q.m);
+		if(q.head - q.tail >= (whole_group ? group_bytes(c, r) : 1u)) return true;
+	}
+	return false;
+}
+
 /* Ragged spans: receiver r brings n_dec[r] decimated samples (host buffer, or device buffer ordered after producer_stream).
  * Everything is checked before the device is touched; the span then runs the chain at its width, the largest count, with
  * the span's receiver table (built in the slot's pinned copy: the slot's previous chunk has been harvested) telling every
@@ -1173,6 +1273,10 @@ static int ragged_submit(vdl2gpu_ctx *c, const void *iq, const uint32_t *n_dec, 
 	}
 	if(width == 0) return VDL2GPU_OK;
 	if(!iq) return VDL2GPU_EINVAL;
+	if(push_queued(c, false)) {          /* those bytes come first in their receivers' streams */
+		snprintf(g_last_error, sizeof(g_last_error), "%s: receivers have pushed bytes not yet in a span (vdl2gpu_submit_pushed first)", what);
+		return VDL2GPU_EINVAL;
+	}
 	CU(cudaSetDevice(c->device));
 	chunk_slot *s;
 	int rc = acquire_slot(c, &s);
@@ -1203,6 +1307,202 @@ extern "C" int vdl2gpu_submit_ragged_device(vdl2gpu_ctx *c, const void *dev_iq, 
 	return ragged_submit(c, dev_iq, n_dec, true, producer_stream, "vdl2gpu_submit_ragged_device");
 }
 
+/* ------------------------------------------------------------------------------------------------
+ * pushed input (vdl2gpu_push, vdl2gpu_submit_pushed; see DESIGN.md, "Pushed input", for the ordering rules)
+ * ---------------------------------------------------------------------------------------------- */
+/* the rings of the current receiver list, their pinned host mirror and empty queues; on failure nothing stays allocated */
+static int alloc_rings_impl(vdl2gpu_ctx *c) {
+	const uint32_t n_rx = c->n_streams;
+	c->rings.resize(n_rx);
+	const uint64_t total = vdl2_push_ring_layout(c->rx_in.data(), n_rx, c->cfg.max_chunk_bytes, c->max_span, c->rings.data());
+	CU(cudaMalloc(&c->d_rings, total));
+	CU(cudaHostAlloc((void **)&c->h_rings, total, cudaHostAllocDefault));
+	CU(cudaMalloc(&c->d_ring_tab, (size_t)n_rx * sizeof(vdl2_rx_ring)));
+	CU(cudaMemcpy(c->d_ring_tab, c->rings.data(), (size_t)n_rx * sizeof(vdl2_rx_ring), cudaMemcpyHostToDevice));
+	c->push.resize(n_rx);
+	for(auto &q : c->push) q.reset(new push_rx());
+	return VDL2GPU_OK;
+}
+
+static int alloc_rings(vdl2gpu_ctx *c) {
+	const int rc = alloc_rings_impl(c);
+	if(rc) free_rings(c);
+	return rc;
+}
+
+/* len bytes at stream position pos of receiver r's ring: into the host mirror, then one copy per piece on stream st */
+static int ring_write(vdl2gpu_ctx *c, cudaStream_t st, uint32_t r, uint64_t pos, const uint8_t *src, uint32_t len) {
+	const vdl2_rx_ring &rg = c->rings[r];
+	const vdl2_ring_segs sg = vdl2_ring_segments(rg.cap, pos, len);
+	for(int k = 0; k < 2; k++) {
+		if(!sg.len[k]) continue;
+		uint8_t *h = c->h_rings + rg.base + sg.off[k];
+		memcpy(h, src, sg.len[k]);
+		CU(cudaMemcpyAsync(c->d_rings + rg.base + sg.off[k], h, sg.len[k], cudaMemcpyHostToDevice, st));
+		src += sg.len[k];
+	}
+	return VDL2GPU_OK;
+}
+
+extern "C" int vdl2gpu_push(vdl2gpu_ctx *c, uint32_t r, const void *iq, uint32_t len) {
+	struct timeval arrival;
+	gettimeofday(&arrival, NULL);
+	const char *why = nullptr;
+	if(!c) why = "no context";
+	else if(!c->ragged) why = "needs a context made by vdl2gpu_create_mixed_receivers with VDL2GPU_FLAG_RAGGED";
+	else if(r >= c->n_streams) why = "no such receiver";
+	else if(!iq && len) why = "no buffer";
+	if(why) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_push: %s", why);
+		return VDL2GPU_EINVAL;
+	}
+	if(len > c->cfg.max_chunk_bytes) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_push: %u bytes, at most max_chunk_bytes = %u", len, c->cfg.max_chunk_bytes);
+		return VDL2GPU_ETOOBIG;
+	}
+	if(len == 0) return VDL2GPU_OK;
+	CU(cudaSetDevice(c->device));
+	if(!c->push_ready) {
+		std::lock_guard<std::mutex> lk(c->push_alloc);
+		if(!c->push_ready) {
+			if(!c->s_copy) {
+				CU(cudaStreamCreateWithFlags(&c->s_copy, cudaStreamNonBlocking));
+				CU(cudaEventCreateWithFlags(&c->ev_copied, cudaEventDisableTiming));
+				CU(cudaEventCreateWithFlags(&c->ev_dropped, cudaEventDisableTiming));
+			}
+			const int rc = alloc_rings(c);
+			if(rc) return rc;
+			c->push_ready = true;
+		}
+	}
+	push_rx &q = *c->push[r];
+	const uint64_t cap = c->rings[r].cap;
+	std::unique_lock<std::mutex> lk(q.m);
+	/* back-pressure: wait until the bytes before `freed` cover enough of the ring.  Fences complete without the caller;
+	 * with none left, only vdl2gpu_submit_pushed (taking the queue into spans, which adds fences) makes room. */
+	while(vdl2_push_room(cap, q.head, q.freed) < len) {
+		while(!q.fences.empty()) {
+			const cudaError_t e = cudaEventQuery(q.fences.front().ev);
+			if(e == cudaErrorNotReady) break;
+			if(e != cudaSuccess) return fail_cuda(e, "cudaEventQuery", __LINE__);
+			q.freed = q.fences.front().pos;
+			q.fences.pop_front();
+		}
+		if(vdl2_push_room(cap, q.head, q.freed) >= len) break;
+		if(!q.fences.empty()) {
+			const cudaEvent_t ev = q.fences.front().ev;
+			lk.unlock();
+			const cudaError_t e = cudaEventSynchronize(ev);
+			lk.lock();
+			if(e != cudaSuccess) return fail_cuda(e, "cudaEventSynchronize", __LINE__);
+		} else {
+			q.room.wait(lk);
+		}
+	}
+	const int rc = ring_write(c, c->s_copy, r, q.head, static_cast<const uint8_t *>(iq), len);
+	if(rc) return rc;
+	/* published only now: the copies are issued, so an event submit_pushed records on the copy stream after reading head
+	 * covers every byte before it */
+	q.head += len;
+	q.recs.push_back({ q.head, (double)arrival.tv_sec + 1e-6 * (double)arrival.tv_usec });
+	return VDL2GPU_OK;
+}
+
+/* vdl2gpu_update_receivers: rings for the new list n beside the old ones in c, each kept receiver's queue moved to its new
+ * index: its partial group (fewer bytes than a group, read from the host mirror of its old ring, written at the same stream
+ * positions of its new ring) and its arrival and span records.  c is left as it was. */
+static int carry_pushed(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const int32_t *from) {
+	int rc = alloc_rings(n);
+	for(uint32_t r = 0; r < n->n_streams && rc == VDL2GPU_OK; r++) {
+		if(from[r] < 0) continue;
+		push_rx &o = *c->push[from[r]], &q = *n->push[r];
+		q.head = o.head; q.tail = q.freed = o.tail;
+		q.recs = o.recs; q.anchors = o.anchors;
+		std::vector<uint8_t> part;
+		const vdl2_rx_ring &rg = c->rings[from[r]];
+		const vdl2_ring_segs sg = vdl2_ring_segments(rg.cap, o.tail, o.head - o.tail);
+		for(int k = 0; k < 2; k++) part.insert(part.end(), c->h_rings + rg.base + sg.off[k], c->h_rings + rg.base + sg.off[k] + sg.len[k]);
+		rc = ring_write(n, c->s_copy, r, q.tail, part.data(), (uint32_t)part.size());
+	}
+	if(rc == VDL2GPU_OK) { cudaError_t e = cudaStreamSynchronize(c->s_copy); if(e != cudaSuccess) rc = fail_cuda(e, "cudaStreamSynchronize", __LINE__); }
+	if(rc) free_rings(n);
+	else n->push_ready = true;
+	return rc;
+}
+
+/* exchange the pushed-input rings (the switch of vdl2gpu_update_receivers; the copy stream stays with the context) */
+static void swap_rings(vdl2gpu_ctx *a, vdl2gpu_ctx *b) {
+	using std::swap;
+	swap(a->d_rings, b->d_rings); swap(a->h_rings, b->h_rings); swap(a->rings, b->rings); swap(a->d_ring_tab, b->d_ring_tab);
+	swap(a->push, b->push);
+	const bool pa = a->push_ready, pb = b->push_ready;
+	a->push_ready = pb; b->push_ready = pa;
+}
+
+/* decimated samples before a receiver's position for which span and arrival records are kept: a burst is harvested at
+ * most n_inflight + 1 spans after the one it completes in, and its sync lies at most one burst before that */
+static uint64_t push_keep_dec(const vdl2gpu_ctx *c) {
+	return (uint64_t)(c->cfg.n_inflight + 2u) * c->max_span + (uint64_t)(VDL2_MAX_BURST_BITS / 3u + 64u) * VDL2_SPS;
+}
+
+extern "C" int vdl2gpu_submit_pushed(vdl2gpu_ctx *c) {
+	if(!c) return VDL2GPU_EINVAL;
+	if(!c->ragged) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_submit_pushed: needs a context made by vdl2gpu_create_mixed_receivers with VDL2GPU_FLAG_RAGGED");
+		return VDL2GPU_EINVAL;
+	}
+	if(!c->push_ready) return 0;
+	CU(cudaSetDevice(c->device));
+	const uint32_t n_rx = c->n_streams;
+	std::vector<uint32_t> take(n_rx);
+	std::vector<uint64_t> tail(n_rx), start(n_rx), limit(n_rx);
+	const uint64_t keep = push_keep_dec(c);
+	/* One snapshot of the heads at entry: every byte before them has its copy issued.  The call drains up to them and no
+	 * further, so it returns however fast other threads keep pushing; bytes pushed meanwhile wait for the next call. */
+	for(uint32_t r = 0; r < n_rx; r++) {
+		push_rx &q = *c->push[r];
+		std::lock_guard<std::mutex> lk(q.m);
+		limit[r] = q.head;
+	}
+	int spans = 0;
+	for(;;) {
+		uint32_t width = 0;
+		for(uint32_t r = 0; r < n_rx; r++) {
+			push_rx &q = *c->push[r];
+			std::lock_guard<std::mutex> lk(q.m);
+			take[r] = vdl2_push_take(limit[r], q.tail, group_bytes(c, r), c->max_span);
+			start[r] = tail[r] = q.tail;
+			width = std::max(width, take[r]);
+		}
+		if(width == 0) break;
+		chunk_slot *s;
+		int rc = acquire_slot(c, &s);
+		if(rc) return rc;
+		/* ... and the front stream waits for those copies */
+		CU(cudaEventRecord(c->ev_copied, c->s_copy));
+		CU(cudaStreamWaitEvent(c->stream, c->ev_copied, 0));
+		vdl2_push_span_table(c->rx_in.data(), c->rings.data(), n_rx, take.data(), tail.data(), c->rx_pos.data(), c->rx_prev.data(), s->h_span);
+		fill_restarts(c, *s);
+		s->pushed = true;
+		rc = run_chain(c, *s, nullptr, width);
+		if(rc) return rc;
+		for(uint32_t r = 0; r < n_rx; r++) {
+			if(!take[r]) continue;
+			push_rx &q = *c->push[r];
+			q.anchors.push_back({ s->h_span[r].dec_base, start[r], take[r] });
+			const uint64_t pos = c->rx_pos[r];
+			while(!q.anchors.empty() && q.anchors.front().dec_base + q.anchors.front().n + keep < pos) q.anchors.pop_front();
+			std::lock_guard<std::mutex> lk(q.m);
+			q.tail = tail[r];
+			q.fences.push_back({ s->k0_done, tail[r] });
+			while(!q.recs.empty() && q.recs.front().end <= q.anchors.front().byte_base) q.recs.pop_front();
+			q.room.notify_all();
+		}
+		spans++;
+	}
+	return spans;
+}
+
 /* Restart receiver r at the start of the next span that runs (see include/vdl2gpu.h).  Only the host's record of the
  * receiver's tuning changes here; the kernels of that span apply the restart, each at its own stage of the pipeline. */
 extern "C" int vdl2gpu_restart_receiver(vdl2gpu_ctx *c, uint32_t r, uint32_t centerfreq, const uint32_t *freqs) {
@@ -1217,6 +1517,20 @@ extern "C" int vdl2gpu_restart_receiver(vdl2gpu_ctx *c, uint32_t r, uint32_t cen
 	if(r >= c->n_streams) {
 		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_restart_receiver: receiver %u of %u", r, c->n_streams);
 		return VDL2GPU_EINVAL;
+	}
+	if(c->push_ready) {
+		/* the old process is killed now: its pushed bytes not yet in a span go with it, a split sample included; the
+		 * receiver's next push starts on a sample boundary.  The dropped bytes' ring places come back once their copies
+		 * are done. */
+		push_rx &q = *c->push[r];
+		std::lock_guard<std::mutex> lk(q.m);
+		if(q.head != q.tail) {
+			CU(cudaSetDevice(c->device));
+			CU(cudaEventRecord(c->ev_dropped, c->s_copy));
+			q.head = q.tail = vdl2_push_realign(q.head, c->rx_in[r].fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
+			q.fences.push_back({ c->ev_dropped, q.head });
+		}
+		q.room.notify_all();
 	}
 	if(centerfreq) c->rx_centre[r] = centerfreq;
 	if(freqs) std::copy(freqs, freqs + (c->rx_first[r + 1] - c->rx_first[r]), c->freqs.begin() + c->rx_first[r]);
@@ -1306,6 +1620,7 @@ extern "C" int vdl2gpu_update_receivers(vdl2gpu_ctx *c, const vdl2gpu_receiver_e
 	if(!c) why = "no context";
 	else if(!c->ragged) why = "needs a context made by vdl2gpu_create_mixed_receivers with VDL2GPU_FLAG_RAGGED";
 	else if(vdl2gpu_chunks_in_flight(c) != 0) why = "spans are in flight (vdl2gpu_flush first)";
+	else if(push_queued(c, true)) why = "receivers have whole decimation groups pushed and not yet in a span (vdl2gpu_submit_pushed first)";
 	else if((why = mixed_count_error(rx, n_rx))) {}
 	else if(!from || !freqs) why = "from and freqs must not be NULL";
 	else if((why = mixed_list_error(rx, n_rx, buf, sizeof(buf), &sum))) {}
@@ -1347,12 +1662,15 @@ extern "C" int vdl2gpu_update_receivers(vdl2gpu_ctx *c, const vdl2gpu_receiver_e
 	n->cfg.n_streams = n_rx;
 	int rc = setup_layout(n, &cfg, base.data(), n_rx, rx, c->n_slots, "vdl2gpu_update_receivers");
 	if(rc == VDL2GPU_OK) rc = migrate_receivers(c, n, rx, from);
+	if(rc == VDL2GPU_OK && c->push_ready) rc = carry_pushed(c, n, from);
 	if(rc == VDL2GPU_OK) {
 		swap_layout(c, n);
+		swap_rings(c, n);
 		/* the graphs went with the old chunk slots: the next spans capture anew, as after create */
 		c->graph_nominal = 0;
 		c->last_n_dec = 0;
 	}
+	free_rings(n);
 	free_layout(n);
 	delete n;
 	return rc;

@@ -138,6 +138,22 @@ __global__ void __launch_bounds__(256) k0_convert_ragged(const uint8_t *__restri
 	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(raw, in, i, levels);
 }
 
+/* K0 on pushed spans: grid row r converts the span[r].n x os_r samples of receiver r where its pushes left them, in its
+ * ring (ring[r]) from ring offset span[r].off on, wrapping at the ring's end, into row r of the sample plane.  The ring's
+ * capacity is a multiple of the sample size and its tail advances in whole groups, so no sample straddles the wrap and
+ * every cs16 sample starts 4-byte aligned. */
+__global__ void __launch_bounds__(256) k0_convert_rings(const uint8_t *__restrict__ rings, const vdl2_rx_input *__restrict__ rx,
+		const vdl2_rx_ring *__restrict__ ring, const vdl2_rx_span *__restrict__ span, const float *__restrict__ levels,
+		float2 *__restrict__ out0, uint32_t out_stride) {
+	const vdl2_rx_input in = rx[blockIdx.y];
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= span[blockIdx.y].n * in.oversample) return;
+	const vdl2_rx_ring rg = ring[blockIdx.y];
+	uint64_t p = span[blockIdx.y].off + (uint64_t)i * (in.fmt == 0 ? 2u : 4u);     /* < 2 cap: a span is shorter than the ring */
+	if(p >= rg.cap) p -= rg.cap;
+	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(rings + rg.base + p, in, 0, levels);
+}
+
 /* ------------------------------------------------------------------------------------------------
  * K1, plain per-sample form (reference for the pipelined kernel; selected by VDL2GPU_FLAG_K1_SCALAR
  * and for oversample values without a specialisation).
@@ -1520,6 +1536,14 @@ extern "C" int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2
 	if(width == 0 || n_rx == 0) return 0;
 	k0_convert_ragged<<<dim3((width * os_max + 255) / 256, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), rx, span, levels,
 			reinterpret_cast<float2 *>(out2), out_stride, ca);
+	return (int)cudaGetLastError();
+}
+
+extern "C" int vdl2_launch_k0_rings(const uint8_t *rings, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_ring *ring, const vdl2_rx_span *span,
+		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, cudaStream_t st) {
+	if(width == 0 || n_rx == 0) return 0;
+	k0_convert_rings<<<dim3((width * os_max + 255) / 256, n_rx), 256, 0, st>>>(rings, rx, ring, span, levels,
+			reinterpret_cast<float2 *>(out2), out_stride);
 	return (int)cudaGetLastError();
 }
 

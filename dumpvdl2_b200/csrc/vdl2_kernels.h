@@ -168,6 +168,10 @@ int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *r
  * (sizes the grid) */
 int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
 		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
+/* pushed spans: row r converts span[r].n x rx[r].oversample samples from receiver r's ring (rings + ring[r].base), starting
+ * at ring offset span[r].off and wrapping at ring[r].cap; width = the largest span[r].n (sizes the grid) */
+int vdl2_launch_k0_rings(const uint8_t *rings, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_ring *ring, const vdl2_rx_span *span,
+		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, cudaStream_t st);
 int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st);
 int vdl2_launch_copy_hist(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k2a(const vdl2_k2_params *p, cudaStream_t st);

@@ -208,6 +208,60 @@ int vdl2gpu_submit_span_device(vdl2gpu_ctx *ctx, const void *dev_iq, uint32_t n_
 int vdl2gpu_submit_ragged(vdl2gpu_ctx *ctx, const void *iq, const uint32_t *n_dec /* [n_rx] */);
 int vdl2gpu_submit_ragged_device(vdl2gpu_ctx *ctx, const void *dev_iq, const uint32_t *n_dec /* [n_rx], host memory */,
 		void *producer_stream);
+/* Pushed input on a ragged mixed-receivers context (VDL2GPU_FLAG_RAGGED): the per-receiver form of the reference's
+ * process_buf_uchar / process_buf_short, one call per device callback.  Any other context returns VDL2GPU_EINVAL.
+ *
+ * vdl2gpu_push(ctx, r, iq, len) queues len bytes of receiver r, in its own format, inside the library.  len may be any
+ * length up to max_chunk_bytes (more: VDL2GPU_ETOOBIG; 0: a no-op); a buffer may end inside a decimation group or inside a
+ * complex sample.  Each receiver decodes exactly what one reference process at its rate decodes from the concatenation of
+ * every byte pushed for it, however the stream was cut, up to the last whole decimation group that has gone into a span.
+ * The caller may reuse iq as soon as the call returns.  VDL2GPU_EINVAL, before the device is touched, for a NULL context,
+ * r >= n_rx, iq NULL with len > 0, or any context but a ragged mixed-receivers one.
+ *   - The bytes go to pinned host memory and are copied at once into the receiver's ring in device memory, on a copy stream
+ *     of the context, so the copy engine moves them while the GPU computes.
+ *   - Back-pressure, as in the reference: a push blocks while its receiver's ring lacks room.  Room comes back when spans
+ *     already in flight have converted their samples (nothing is needed from the caller for that) and when
+ *     vdl2gpu_submit_pushed takes queued bytes into spans.  A push of up to max_chunk_bytes that follows a
+ *     vdl2gpu_submit_pushed never waits for the caller, only for the GPU: a single thread that alternates pushes and
+ *     vdl2gpu_submit_pushed cannot deadlock.
+ *   - Memory: the first push allocates every receiver's ring, max_chunk_bytes + (max_span + 1) x oversample_r x bytes per
+ *     complex sample_r bytes (rounded up to 16), in device memory and again in pinned host memory; contexts that never push
+ *     pay nothing.  For 2048 receivers at the default 1 MiB that is up to about 4 GiB of each (a cs16 receiver at oversample
+ *     20: 2 MiB).  An allocation failure is returned by that first push.
+ *   - Each push records its arrival time (gettimeofday at entry) for the burst timestamps below.
+ *
+ * vdl2gpu_submit_pushed(ctx) reads every receiver's queue once, when it is entered, and submits ragged spans until every
+ * whole decimation group queued at that moment is in a span.  Bytes pushed during the call wait for the next call, so the
+ * call returns however fast other threads keep pushing, and a control loop of submit_pushed and poll keeps delivering
+ * frames.  Each span takes min(whole groups left of that snapshot, max_span) from every receiver, so a receiver far behind
+ * catches up over several spans.  Returns the number of spans submitted (0 when nothing was queued: a no-op that leaves restarts pending)
+ * or a negative error.  Frames come out through vdl2gpu_poll / vdl2gpu_flush as for any span (vdl2gpu_flush forms no
+ * spans).  Positions, stats.iq_samples, dec_samples and chunks_submitted count exactly as for vdl2gpu_submit_ragged spans
+ * of the same counts.
+ *
+ * Burst timestamps of pushed spans: the arrival time of the push that carried the last input sample of the burst's sync
+ * decimation group, moved back by the input samples that push carried after that sample, at the receiver's own rate (the
+ * receiver's analogue of the reference stamping at processing time; it does not depend on when vdl2gpu_submit_pushed runs).
+ *
+ * Threads: vdl2gpu_push may run concurrently for different receivers, and concurrently with vdl2gpu_submit_pushed,
+ * vdl2gpu_poll, vdl2gpu_flush and vdl2gpu_get_stats on the one control thread.  Two pushes of the same receiver are
+ * serialised, in an unspecified order: keep one thread per receiver.  No push may run during vdl2gpu_update_receivers or
+ * vdl2gpu_destroy, and no push of receiver r during vdl2gpu_restart_receiver(ctx, r, ...).
+ *
+ * With the other calls:
+ *   - vdl2gpu_submit_ragged*, vdl2gpu_submit_span* return VDL2GPU_EINVAL while any receiver has pushed bytes not yet in a
+ *     span (stream order); with nothing queued the two ways of feeding may alternate.
+ *   - vdl2gpu_restart_receiver(r) drops r's pushed bytes not yet in a span, a split sample included (the old process is
+ *     killed at the call); the restart applies at the next span as always, and bytes pushed after the call belong to the
+ *     new process.  Call vdl2gpu_submit_pushed first to have the queued groups decoded.
+ *   - vdl2gpu_update_receivers also refuses (VDL2GPU_EINVAL) while any receiver has a whole group queued.  A kept receiver
+ *     carries its partial group (fewer than oversample_r samples, or a split sample) and its arrival records to its new
+ *     index; a removed receiver's bytes are dropped; a new receiver starts empty.  Once anything has been pushed, the call
+ *     allocates the new list's rings before it frees the old ones, so for the call's duration the device and the pinned
+ *     host memory briefly hold both sets of rings (up to about 2 x 4 GiB of each for 2048 receivers at the default
+ *     max_chunk_bytes), on top of the rebuild described below. */
+int vdl2gpu_push(vdl2gpu_ctx *ctx, uint32_t r, const void *iq, uint32_t len);
+int vdl2gpu_submit_pushed(vdl2gpu_ctx *ctx);
 /* out[r] = decimated samples of receiver r accepted so far, for the first n_rx receivers of a receivers context (with ragged
  * spans: the sum of receiver r's counts, which shows which receiver lags; in lock step all receivers are equal) */
 int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *ctx, uint64_t *out, uint32_t n_rx);
