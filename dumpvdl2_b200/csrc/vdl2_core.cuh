@@ -641,6 +641,35 @@ VDL2_HD void vdl2_walk_tail(vdl2_chan &v, float *ring, int rs, const vdl2_k2_env
 	}
 }
 
+/* The searching path reads and writes the ring at one of two positions per block (before and after the wrap at 160)
+ * plus a compile-time offset.  vdl2_ring_at(ring, i) is the position of ring[i], vdl2_ring_ld / vdl2_ring_st access
+ * ring[i + k] from it.  On the device the position is the 32-bit shared-memory address of ring[i], hidden from the
+ * compiler's value tracking, so that picking one of two positions is one select and the access folds k into its
+ * immediate: written as indices, the select is rewritten into a select of indices followed, per access, by the
+ * arithmetic both positions share (the lane's column, the scaling, the ring's base).  ring is the lane's column of the
+ * shared-memory ring there; on the host the position is the index itself. */
+#ifdef __CUDA_ARCH__
+typedef uint32_t vdl2_ring_pos;
+VDL2_HD vdl2_ring_pos vdl2_ring_at(const float *ring, int i) {
+	uint32_t a = (uint32_t)__cvta_generic_to_shared(ring) + 4u * (uint32_t)i;
+	asm("" : "+r"(a));
+	return a;
+}
+VDL2_HD float vdl2_ring_ld(const float *, vdl2_ring_pos a, int k) {
+	float x;
+	asm("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(a + 4u * (uint32_t)k) : "memory");
+	return x;
+}
+VDL2_HD void vdl2_ring_st(float *, vdl2_ring_pos a, int k, float x) {
+	asm volatile("st.shared.f32 [%0], %1;" :: "r"(a + 4u * (uint32_t)k), "f"(x) : "memory");
+}
+#else
+typedef int vdl2_ring_pos;
+VDL2_HD vdl2_ring_pos vdl2_ring_at(const float *, int i) { return i; }
+VDL2_HD float vdl2_ring_ld(const float *ring, vdl2_ring_pos a, int k) { return ring[a + k]; }
+VDL2_HD void vdl2_ring_st(float *ring, vdl2_ring_pos a, int k, float x) { ring[a + k] = x; }
+#endif
+
 template<bool STAGED = false>
 VDL2_HD void vdl2_walk_block_ring(vdl2_chan &v, float *ring, int rs, const vdl2_k2_env &env, uint32_t chan_idx, uint64_t idx0,
 		const float2 *dec, const float *phase, const float *mag, size_t stride, vdl2_walk_pref &pf, bool has_next) {
@@ -678,16 +707,19 @@ VDL2_HD void vdl2_walk_block_ring(vdl2_chan &v, float *ring, int rs, const vdl2_
 	int resume = 0;
 	if(fast) {
 		float ph[4][VDL2_PREAMBLE_SYMS], p0[4], sl[4];
+		/* slot of sample e-150 with e = first + 3j: P + 1 + e - 150 == P + e + 11 (mod 160).  With b = that slot for j = 0,
+		 * read i of attempt j is slot b + o, o = 3j + 10i <= 149, and b + o < 320: the ring wraps at most once over all 60
+		 * reads, so each is one of two positions (before / after the wrap) plus a compile-time offset, picked by one
+		 * compare against an immediate. */
+		int b = v.ring_pos + first + 11;
+		if(b >= VDL2_SYNC_BUFLEN) b -= VDL2_SYNC_BUFLEN;
+		const vdl2_ring_pos rd_lo = vdl2_ring_at(ring, b * rs), rd_hi = vdl2_ring_at(ring, (b - VDL2_SYNC_BUFLEN) * rs);
 #pragma unroll
 		for(int j = 0; j < 4; j++) {
-			/* slot of sample e-150 with e = first + 3j: P + 1 + e - 150 == P + e + 11 (mod 160) */
-			int idx = v.ring_pos + first + VDL2_SYNC_SKIP * j + 11;
-			if(idx >= VDL2_SYNC_BUFLEN) idx -= VDL2_SYNC_BUFLEN;
 #pragma unroll
 			for(int i = 0; i < VDL2_PREAMBLE_SYMS - 1; i++) {
-				ph[j][i] = ring[idx * rs];
-				idx += VDL2_SPS;
-				if(idx >= VDL2_SYNC_BUFLEN) idx -= VDL2_SYNC_BUFLEN;
+				const int o = VDL2_SYNC_SKIP * j + VDL2_SPS * i;
+				ph[j][i] = vdl2_ring_ld(ring, b < VDL2_SYNC_BUFLEN - o ? rd_lo : rd_hi, o * rs);
 			}
 			/* i = 15 is the attempt's own sample, one of the block's inputs */
 			ph[j][15] = (first == 0) ? pw[VDL2_SYNC_SKIP * j] : ((first == 1) ? pw[VDL2_SYNC_SKIP * j + 1] : pw[VDL2_SYNC_SKIP * j + 2]);
@@ -698,17 +730,23 @@ VDL2_HD void vdl2_walk_block_ring(vdl2_chan &v, float *ring, int rs, const vdl2_
 		vdl2_metric_core_n<4, true>(ph, env.pr_phase, env.lr_X, env.lr_denom, env.unwrap_lut, p0, sl);
 		const int sclk_entry = v.sclk;
 		/* The twelve ring slots of the block follow from the entry position (vdl2_init_write advances by one with a
-		 * wrap at 160): slot of sample t = wrap(entry + 1 + t), each computed on its own instead of as a chain of
-		 * twelve dependent updates; the saturating run counter is advanced once, by the number of samples written. */
+		 * wrap at 160): slot of sample t = entry + 1 + t, wrapped at most once over the block (entry + 1 + 11 < 320), so
+		 * each store is one of two positions plus a compile-time offset, like the reads above; the saturating run
+		 * counter is advanced once, by the number of samples written. */
 		const int rp_entry = v.ring_pos + 1;
+		const vdl2_ring_pos wr_lo = vdl2_ring_at(ring, rp_entry * rs), wr_hi = vdl2_ring_at(ring, (rp_entry - VDL2_SYNC_BUFLEN) * rs);
 #define VDL2_RING_SLOT(t) ((rp_entry + (t)) >= VDL2_SYNC_BUFLEN ? (rp_entry + (t)) - VDL2_SYNC_BUFLEN : (rp_entry + (t)))
+#define VDL2_RING_PUT(t) vdl2_ring_st(ring, rp_entry < VDL2_SYNC_BUFLEN - (t) ? wr_lo : wr_hi, (t) * rs, pw[t])
+		/* which of a group's three samples precede its attempt (u <= first), decided once for the block */
+		static_assert(VDL2_SYNC_SKIP == 3, "a group is three samples");
+		const bool pre1 = first >= 1, pre2 = first >= 2;
 		bool go = true;
 #pragma unroll
 		for(int g = 0; g < 4; g++) {
 			if(go) {
-#pragma unroll
-				for(int u = 0; u < VDL2_SYNC_SKIP; u++)
-					if(u <= first) ring[VDL2_RING_SLOT(VDL2_SYNC_SKIP * g + u) * rs] = pw[VDL2_SYNC_SKIP * g + u];
+				VDL2_RING_PUT(VDL2_SYNC_SKIP * g);
+				if(pre1) VDL2_RING_PUT(VDL2_SYNC_SKIP * g + 1);
+				if(pre2) VDL2_RING_PUT(VDL2_SYNC_SKIP * g + 2);
 				v.ring_pos = VDL2_RING_SLOT(VDL2_SYNC_SKIP * g + first);
 				v.sclk = 0;
 				vdl2_init_eval(v, ring, rs, env, chan_idx, idx0 + (uint64_t)(VDL2_SYNC_SKIP * g + first), mg[g], true, p0[g], sl[g]);
@@ -716,14 +754,14 @@ VDL2_HD void vdl2_walk_block_ring(vdl2_chan &v, float *ring, int rs, const vdl2_
 					go = false;                      /* locked, or vetoed by max_ppm: the per-sample path takes over */
 					resume = VDL2_SYNC_SKIP * g + first + 1;
 				} else {
-#pragma unroll
-					for(int u = 0; u < VDL2_SYNC_SKIP; u++)
-						if(u > first) ring[VDL2_RING_SLOT(VDL2_SYNC_SKIP * g + u) * rs] = pw[VDL2_SYNC_SKIP * g + u];
+					if(!pre1) VDL2_RING_PUT(VDL2_SYNC_SKIP * g + 1);
+					if(!pre2) VDL2_RING_PUT(VDL2_SYNC_SKIP * g + 2);
 					v.ring_pos = VDL2_RING_SLOT(VDL2_SYNC_SKIP * g + VDL2_SYNC_SKIP - 1);
 					v.sclk = sclk_entry;
 				}
 			}
 		}
+#undef VDL2_RING_PUT
 #undef VDL2_RING_SLOT
 		if(go) resume = VDL2_WALK_BLOCK;
 		{
