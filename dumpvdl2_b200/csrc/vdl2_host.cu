@@ -1838,7 +1838,9 @@ extern "C" int vdl2gpu_read_dec(vdl2gpu_ctx *c, float *out, size_t cap_floats, u
 	*n_dec = c->last_n_dec;
 	if((size_t)c->last_n_dec * c->n_ch * 2 > cap_floats) return VDL2GPU_ETOOBIG;
 	if(c->last_n_dec == 0) return VDL2GPU_OK;
-	if(c->lanes == 32) {
+	/* slot == channel only without the balanced mapping, which can deal 32 channels (lanes == 32) to the first full_warps
+	 * warps and 31 to the others */
+	if(c->full_warps == 0xFFFFFFFFu) {
 		CU(cudaMemcpy2D(out, (size_t)c->n_ch * sizeof(float2), c->d_dec3[(c->chunk_seq + 2) % 3u], (size_t)c->n_chp * sizeof(float2),
 				(size_t)c->n_ch * sizeof(float2), c->last_n_dec, cudaMemcpyDeviceToHost));
 	} else {
