@@ -15,6 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvdl2gpu.so")
 FMT_U8, FMT_S16 = 0, 1
 FLAG_TRACE, FLAG_KEEP_DEC, FLAG_K1_SCALAR, FLAG_NO_OVERLAP, FLAG_NO_GRAPH, FLAG_RAGGED = 1, 2, 4, 8, 16, 32
+FLAG_INPUT_LEVELS = 64
 NUM_COUNTERS = 9
 COUNTER_NAMES = ["sync_good", "hdr_crc_good", "bursts", "burst_err", "blocks_processed",
                  "blocks_fec_ok", "msg_good", "fcs_good", "fcs_bad"]
@@ -57,6 +58,11 @@ class _Stats(C.Structure):
                 ("chunks_submitted", "chunks_completed", "iq_samples", "dec_samples", "demod_sync_good",
                  "decoder_crc_good", "bursts", "burst_errors", "blocks_processed", "blocks_fec_ok", "msg_good",
                  "fcs_good", "fcs_bad", "pool_overflows", "out_overflows", "kernel_launches", "out_bytes", "graph_launches")] + [("reserved", C.c_uint64 * 2)]
+
+
+class _InputLevels(C.Structure):
+    _fields_ = [("samples", C.c_uint64), ("sum_i", C.c_int64), ("sum_q", C.c_int64), ("pow_lo", C.c_uint64),
+                ("pow_hi", C.c_uint64), ("clipped", C.c_uint64), ("peak", C.c_uint32), ("full_scale", C.c_uint32)]
 
 
 class _Event(C.Structure):
@@ -106,6 +112,7 @@ def load_library():
     L.vdl2gpu_flush.argtypes = [C.c_void_p, _FRAME_CB, C.c_void_p]
     L.vdl2gpu_get_stats.argtypes = [C.c_void_p, C.POINTER(_Stats)]
     L.vdl2gpu_get_channel_counters.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.vdl2gpu_get_input_levels.argtypes = [C.c_void_p, C.POINTER(_InputLevels), C.c_uint32]
     L.vdl2gpu_get_tables.argtypes = [C.c_void_p] + [C.c_void_p] * 8
     L.vdl2gpu_read_dec.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]
     L.vdl2gpu_read_events.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
@@ -188,6 +195,18 @@ def frame_from_c(f):
     return o
 
 
+def level_metrics(rec):
+    """What an operator reads off one record of input_levels(): mean power in dBFS (10 log10 of the mean of c_I^2 + c_Q^2
+    over full_scale^2; -inf for an all-zero input), the DC offsets of I and Q and the peak in full-scale units, and the
+    fraction of samples with a component on a rail.  All None for an input that has measured nothing yet."""
+    n, fs = int(rec["samples"]), int(rec["full_scale"])
+    if n == 0:
+        return dict(power_dbfs=None, dc_i=None, dc_q=None, clipped_fraction=None, peak=None)
+    pw = int(rec["pow"]) / (n * fs * fs)
+    return dict(power_dbfs=10.0 * np.log10(pw) if pw > 0 else float("-inf"), dc_i=int(rec["sum_i"]) / (n * fs),
+                dc_q=int(rec["sum_q"]) / (n * fs), clipped_fraction=int(rec["clipped"]) / n, peak=int(rec["peak"]) / fs)
+
+
 def make_config(sample_rate, oversample, sample_fmt, centerfreq, freqs, max_ppm=0.0, flags=0):
     """(vdl2gpu_config, the freqs array it points at) for the stage stubs"""
     fr = np.ascontiguousarray(freqs, dtype=np.uint32)
@@ -213,9 +232,11 @@ class Vdl2Channels:
     """N VDL2 channels demodulated from one IQ stream on one H100."""
 
     def __init__(self, sample_rate, oversample, sample_fmt, centerfreq, freqs, max_ppm=0.0,
-                 max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, n_streams=1):
+                 max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, n_streams=1, levels=False):
         """n_streams > 1: independent-streams mode, channels [s*C, (s+1)*C) demodulate stream s; process_buf_* then take
-        the S per-stream buffers back to back."""
+        the S per-stream buffers back to back.  levels=True: measure every input's levels (input_levels())."""
+        if levels:
+            flags |= FLAG_INPUT_LEVELS
         self.L = load_library()
         self.n_streams = int(n_streams)
         self.freqs = np.ascontiguousarray(freqs, dtype=np.uint32)
@@ -352,6 +373,17 @@ class Vdl2Channels:
         n = _check(self.L, self.L.vdl2gpu_debug_block_trace(self.h, a.ctypes.data, cap), "vdl2gpu_debug_block_trace")
         return a[:n]
 
+    def input_levels(self):
+        """one dict per input (the stream; the n_streams streams; the receivers, in order) of the exact integers the device
+        measured over every sample submitted so far: samples, sum_i, sum_q, pow (the 128-bit sum of c_I^2 + c_Q^2 as a
+        Python int), clipped, peak, full_scale (see vdl2gpu_get_input_levels; level_metrics() turns one into dBFS and
+        full-scale units).  Needs levels=True at creation."""
+        n = self.n_streams
+        out = (_InputLevels * max(n, 1))()
+        _check(self.L, self.L.vdl2gpu_get_input_levels(self.h, out, n), "vdl2gpu_get_input_levels")
+        return [dict(samples=o.samples, sum_i=o.sum_i, sum_q=o.sum_q, pow=(o.pow_hi << 64) | o.pow_lo, clipped=o.clipped,
+                     peak=o.peak, full_scale=o.full_scale) for o in out[:n]]
+
     def kernel_ms(self):
         ms = (C.c_double * 5)()
         n = (C.c_uint64 * 5)()
@@ -365,8 +397,10 @@ class Vdl2Receivers(Vdl2Channels):
     channels_of(r).  The receivers advance in lock step: submit() takes one equal-length buffer per receiver."""
 
     def __init__(self, sample_rate, oversample, sample_fmt, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1,
-                 flags=0, n_inflight=4):
-        """receivers: list of (centerfreq, [channel freqs...])"""
+                 flags=0, n_inflight=4, levels=False):
+        """receivers: list of (centerfreq, [channel freqs...]); levels=True: measure every receiver's input levels"""
+        if levels:
+            flags |= FLAG_INPUT_LEVELS
         self.L = load_library()
         self.receivers = [(int(cf), [int(f) for f in fr]) for cf, fr in receivers]
         self.n_receivers = self.n_streams = len(self.receivers)
@@ -428,10 +462,14 @@ class Vdl2MixedReceivers(Vdl2Receivers):
     reconnect, a swapped device, a retune) without disturbing the others, and update_receivers() / add_receivers() /
     remove_receivers() let receivers join and leave (after flush()) while the others carry on."""
 
-    def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, ragged=False):
-        """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16))"""
+    def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, ragged=False,
+                 levels=False):
+        """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16));
+        levels=True: measure every receiver's input levels (input_levels())"""
         if ragged:
             flags |= FLAG_RAGGED
+        if levels:
+            flags |= FLAG_INPUT_LEVELS
         self.ragged = bool(flags & FLAG_RAGGED)
         self.L = load_library()
         rxs = self._normalise(receivers)

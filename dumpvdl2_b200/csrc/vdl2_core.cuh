@@ -1522,4 +1522,37 @@ VDL2_HD double vdl2_push_back_seconds(uint64_t sample_end, uint64_t push_end, ui
 	return (double)((push_end - sample_end) / bpp) / (double)rate;
 }
 
+/* ------------------------------------------------------------------------------------------------
+ * Input levels (VDL2GPU_FLAG_INPUT_LEVELS): exact integer figures of every raw sample K0 converts.  A component's code c
+ * is an integer whose ratio to the format's full scale is exactly the float the reference makes of it: cu8 c = 2v - 255
+ * (c / 255 = (v - 127.5) / 127.5, src/demod.c:349-354), cs16 c = v (c / 32768, src/demod.c:361-363).  Formats as K0
+ * takes them: 0 cu8, 1 interleaved cs16, 2 planar cs16.
+ * ---------------------------------------------------------------------------------------------- */
+/* per input, in device memory: the layout of vdl2gpu_input_levels (full_scale is filled in by the getter) */
+typedef struct {
+	uint64_t samples;
+	uint64_t sum_i, sum_q;       /* int64 sums kept as two's complement, so that unsigned 64-bit atomics can add to them */
+	uint64_t pow_lo, pow_hi;
+	uint64_t clipped;
+	uint32_t peak, full_scale;
+} vdl2_levels;
+
+VDL2_HD int32_t vdl2_level_code(uint32_t fmt, int32_t v) { return fmt == 0u ? 2 * v - 255 : v; }
+VDL2_HD uint32_t vdl2_level_rail(uint32_t fmt, int32_t v) { return fmt == 0u ? (v == 0 || v == 255) : (v == -32768 || v == 32767); }
+VDL2_HD uint32_t vdl2_level_mag(int32_t c) { return c < 0 ? (uint32_t)(-c) : (uint32_t)c; }
+VDL2_HD uint32_t vdl2_level_full_scale(uint32_t fmt) { return fmt == 0u ? 255u : 32768u; }
+/* c_I^2 + c_Q^2 of one complex sample: at most 2 x 32768^2 = 2^31 */
+VDL2_HD uint32_t vdl2_level_pow(int32_t ci, int32_t cq) { return (uint32_t)(ci * ci) + (uint32_t)(cq * cq); }
+
+/* The 128-bit sum of squares: a 64-bit addend v goes into (lo, hi).  lo + v wraps exactly when the sum comes out below v,
+ * and then hi takes the carry.  The device does the same with an atomic add on lo, whose return value is the old lo: every
+ * addend carries exactly once when it wraps lo, whatever order the blocks of a chunk add in, so the total is exact and
+ * deterministic with any number of writers. */
+VDL2_HD uint32_t vdl2_pow_carry(uint64_t old_lo, uint64_t v) { return old_lo + v < v ? 1u : 0u; }
+VDL2_HD void vdl2_pow_fold(uint64_t &lo, uint64_t &hi, uint64_t v) {
+	const uint64_t old = lo;
+	lo = old + v;
+	hi += vdl2_pow_carry(old, v);
+}
+
 #endif

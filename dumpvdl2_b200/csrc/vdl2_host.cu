@@ -186,6 +186,9 @@ struct vdl2gpu_ctx {
 	cudaStream_t s_copy = nullptr;
 	cudaEvent_t ev_copied = nullptr, ev_dropped = nullptr;
 	std::vector<std::unique_ptr<push_rx>> push;
+	/* input levels (VDL2GPU_FLAG_INPUT_LEVELS; NULL otherwise): one accumulator per input (stream or receiver), which the
+	 * levels form of K0 adds every converted sample to */
+	vdl2_levels *d_levels = nullptr;
 };
 
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
@@ -245,6 +248,7 @@ static void free_layout(vdl2gpu_ctx *c) {
 	cudaFree(c->d_counters); cudaFree(c->d_ready); cudaFree(c->d_ring); cudaFree(c->d_pool); cudaFree(c->d_free); cudaFree(c->d_ctl);
 	cudaFree(c->d_slot_rx); cudaFree(c->d_block_rx);
 	cudaFree(c->d_rx_in); cudaFree(c->d_slot_cls);
+	cudaFree(c->d_levels);
 }
 
 /* the pushed-input rings and their queues (no push, copy or span may be running on them) */
@@ -419,6 +423,10 @@ static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu
 		CU(cudaMemcpy(c->d_slot_rx, slot_rx.data(), slot_rx.size() * 4, cudaMemcpyHostToDevice));
 		CU(cudaMemcpy(c->d_block_rx, block_rx.data(), block_rx.size() * 4, cudaMemcpyHostToDevice));
 	}
+	if(c->cfg.flags & VDL2GPU_FLAG_INPUT_LEVELS) {
+		CU(cudaMalloc(&c->d_levels, (size_t)c->n_streams * sizeof(vdl2_levels)));
+		CU(cudaMemset(c->d_levels, 0, (size_t)c->n_streams * sizeof(vdl2_levels)));
+	}
 	if(c->mixed) {
 		CU(cudaMalloc(&c->d_rx_in, c->rx_in.size() * sizeof(vdl2_rx_input)));
 		CU(cudaMalloc(&c->d_slot_cls, slot_cls.size()));
@@ -468,6 +476,7 @@ static void swap_layout(vdl2gpu_ctx *a, vdl2gpu_ctx *b) {
 	swap(a->d_samples, b->d_samples); swap(a->d_dec3, b->d_dec3); swap(a->d_phase2, b->d_phase2); swap(a->d_mag2, b->d_mag2);
 	swap(a->d_k1, b->d_k1); swap(a->d_k2, b->d_k2); swap(a->d_counters, b->d_counters); swap(a->d_ring, b->d_ring);
 	swap(a->d_pool, b->d_pool); swap(a->d_free, b->d_free); swap(a->d_ready, b->d_ready); swap(a->d_ctl, b->d_ctl);
+	swap(a->d_levels, b->d_levels);
 	swap(a->chunks, b->chunks);
 }
 
@@ -929,7 +938,7 @@ static inline uint32_t chain_os(const vdl2gpu_ctx *c) { return c->mixed ? 1u : c
 /* mixed-rate receivers: K0 of a span of n_dec decimated samples into the sample plane (ca: graph replay) */
 static int launch_k0_mixed(vdl2gpu_ctx *c, const void *d_raw, uint32_t n_dec, const vdl2_chunk_args *ca) {
 	KL(vdl2_launch_k0_mixed(d_raw, n_dec, c->d_rx_in, c->n_streams, c->rx_os_max, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples),
-			c->max_pairs, ca, c->stream));
+			c->max_pairs, ca, c->d_levels, c->stream));
 	return VDL2GPU_OK;
 }
 
@@ -938,11 +947,11 @@ static int launch_k0_span(vdl2gpu_ctx *c, const chunk_slot &s, const void *d_raw
 	if(!c->ragged) return launch_k0_mixed(c, d_raw, n_dec, ca);
 	if(s.pushed) {                                      /* (never captured: pushed spans take the direct path) */
 		KL(vdl2_launch_k0_rings(c->d_rings, n_dec, c->d_rx_in, c->d_ring_tab, s.d_span, c->n_streams, c->rx_os_max, c->d_tab->levels,
-				reinterpret_cast<float *>(c->d_samples), c->max_pairs, c->stream));
+				reinterpret_cast<float *>(c->d_samples), c->max_pairs, c->d_levels, c->stream));
 		return VDL2GPU_OK;
 	}
 	KL(vdl2_launch_k0_ragged(d_raw, n_dec, c->d_rx_in, s.d_span, c->n_streams, c->rx_os_max, c->d_tab->levels,
-			reinterpret_cast<float *>(c->d_samples), c->max_pairs, ca, c->stream));
+			reinterpret_cast<float *>(c->d_samples), c->max_pairs, ca, c->d_levels, c->stream));
 	return VDL2GPU_OK;
 }
 
@@ -962,9 +971,9 @@ static int body_front(void *a) {
 	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
 	if(c->mixed) { int rc = launch_k0_span(c, *e->s, nullptr, e->n_pairs, e->s->d_args); if(rc) return rc; }
 	else if(c->lane_streams) KL(vdl2_launch_k0_lanes(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-			e->n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, e->s->d_args, c->stream));
+			e->n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, e->s->d_args, c->d_levels, c->stream));
 	else KL(vdl2_launch_k0(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-			e->n_pairs * bpp, c->max_pairs, e->s->d_args, c->stream));
+			e->n_pairs * bpp, c->max_pairs, e->s->d_args, c->d_levels, c->stream));
 	KL(vdl2_launch_k1(&p1, (c->cfg.flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->stream));
 	return 0;
 }
@@ -1041,9 +1050,9 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 			if(rc) return rc;
 			if(s.pushed) CU(cudaEventRecord(s.k0_done, c->stream));     /* the rings' bytes of this span are read */
 		} else if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-				n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, nullptr, c->stream));
+				n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, nullptr, c->d_levels, c->stream));
 		else KL(vdl2_launch_k0(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-				n_pairs * bpp, c->max_pairs, nullptr, c->stream));
+				n_pairs * bpp, c->max_pairs, nullptr, c->d_levels, c->stream));
 		if(s.timed) CU(cudaEventRecord(s.tk[1], c->stream));
 		KL(vdl2_launch_k1(&p1, (c->cfg.flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->stream));
 	}
@@ -1598,6 +1607,16 @@ static int migrate_receivers(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const vdl2gpu_recei
 	CU(cudaMemcpyAsync(n->d_pool, c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot), cudaMemcpyDeviceToDevice, c->stream));
 	CU(cudaMemcpyAsync(n->d_free, fl.data(), fl.size() * 4, cudaMemcpyHostToDevice, c->stream));
 	CU(cudaMemcpyAsync(n->d_ctl, &ctl, sizeof(ctl), cudaMemcpyHostToDevice, c->stream));
+	/* input levels: a kept receiver carries its accumulator to its new index, a new one starts at zero (setup_layout) */
+	std::vector<vdl2_levels> old_lv, new_lv;
+	if(c->d_levels) {
+		old_lv.resize(c->n_streams);
+		new_lv.assign(n_rx, vdl2_levels());
+		CU(cudaMemcpyAsync(old_lv.data(), c->d_levels, old_lv.size() * sizeof(vdl2_levels), cudaMemcpyDeviceToHost, c->stream));
+		CU(cudaStreamSynchronize(c->stream));
+		for(uint32_t r = 0; r < n_rx; r++) if(from[r] >= 0) new_lv[r] = old_lv[from[r]];
+		CU(cudaMemcpyAsync(n->d_levels, new_lv.data(), new_lv.size() * sizeof(vdl2_levels), cudaMemcpyHostToDevice, c->stream));
+	}
 	CU(cudaStreamSynchronize(c->stream));
 	/* per receiver: a kept one carries its position and a pending restart over; every history now starts at row 0 */
 	for(uint32_t r = 0; r < n_rx; r++) {
@@ -1812,6 +1831,35 @@ extern "C" int vdl2gpu_get_channel_counters(vdl2gpu_ctx *c, uint64_t *out, uint3
 	return VDL2GPU_OK;
 }
 
+/* Input levels (VDL2GPU_FLAG_INPUT_LEVELS): out[k] for the first n inputs, after everything submitted so far has run */
+extern "C" int vdl2gpu_get_input_levels(vdl2gpu_ctx *c, vdl2gpu_input_levels *out, uint32_t n) {
+	const char *why = nullptr;
+	if(!c) why = "no context";
+	else if(!out) why = "no output";
+	else if(!c->d_levels) why = "the context was created without VDL2GPU_FLAG_INPUT_LEVELS";
+	else if(n > c->n_streams) why = "more inputs asked for than the context has";
+	if(why) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_get_input_levels: %s", why);
+		return VDL2GPU_EINVAL;
+	}
+	if(n == 0) return VDL2GPU_OK;
+	CU(cudaSetDevice(c->device));
+	CU(cudaStreamSynchronize(c->stream));
+	CU(cudaStreamSynchronize(c->s_back));
+	std::vector<vdl2_levels> lv(n);
+	CU(cudaMemcpy(lv.data(), c->d_levels, (size_t)n * sizeof(vdl2_levels), cudaMemcpyDeviceToHost));
+	for(uint32_t k = 0; k < n; k++) {
+		vdl2gpu_input_levels &o = out[k];
+		o.samples = lv[k].samples;
+		o.sum_i = (int64_t)lv[k].sum_i; o.sum_q = (int64_t)lv[k].sum_q;
+		o.pow_lo = lv[k].pow_lo; o.pow_hi = lv[k].pow_hi;
+		o.clipped = lv[k].clipped;
+		o.peak = lv[k].peak;
+		o.full_scale = vdl2_level_full_scale(c->mixed ? c->rx_in[k].fmt : c->cfg.sample_fmt);
+	}
+	return VDL2GPU_OK;
+}
+
 extern "C" int vdl2gpu_get_tables(vdl2gpu_ctx *c, float levels[256], float sin_lut[257], float cos_lut[257],
 		float A[3], float B[3], float lr_X[16], float *lr_denom, float pr_phase[16]) {
 	if(!c) return VDL2GPU_EINVAL;
@@ -1959,7 +2007,7 @@ static int stub_tables(vdl2_tables **out) {
 extern "C" int vdl2gpu_launch_convert(const void *raw, uint32_t n_pairs, uint32_t sample_fmt, const float *levels256,
 		float *samples_out, void *stream) {
 	if(!raw || !samples_out || sample_fmt > 1 || (sample_fmt == 0 && !levels256)) return VDL2GPU_EINVAL;
-	KL(vdl2_launch_k0(raw, n_pairs, sample_fmt, levels256, samples_out, 1, 0, 0, nullptr, (cudaStream_t)stream));
+	KL(vdl2_launch_k0(raw, n_pairs, sample_fmt, levels256, samples_out, 1, 0, 0, nullptr, nullptr, (cudaStream_t)stream));
 	return VDL2GPU_OK;
 }
 

@@ -37,13 +37,80 @@ __device__ __forceinline__ void vdl2_trace_end(vdl2_block_trace *t, int k) { if(
 /* ------------------------------------------------------------------------------------------------
  * K0: sample conversion.  Output: float2 {re, im} per complex sample (src/demod.c:339-365).
  * ---------------------------------------------------------------------------------------------- */
+/* K0 levels form (VDL2GPU_FLAG_INPUT_LEVELS): every converted sample's integer codes (vdl2_level_code) are also reduced
+ * into the per-input accumulators of vdl2_levels.  A thread of the levels form converts K0_LV_SPT samples (a lanes block
+ * K0_LV_SPT tiles) and sums them in registers; a warp adds its lanes with __reduce_add_sync (the sum of squares as two
+ * halves, below and above bit 16, each of which fits 32 bits over a warp), a block its warps through shared memory, and
+ * one thread issues one integer atomic per field.  Integer atomics commute, so the figures do not depend on the order
+ * the blocks run in; covering K0_LV_SPT samples per thread keeps the atomics on one input's accumulator rare enough not
+ * to queue behind each other. */
+#define K0_LV_SPT 16
+
+struct k0_level_part {
+	int32_t si, sq;              /* sums of the codes (a block: at most 256 x K0_LV_SPT x 32768 in magnitude) */
+	uint64_t pow;                /* (a thread: at most K0_LV_SPT x 2^31) */
+	uint32_t nc;                 /* samples in bits 0..15, clipped samples in bits 16..31 (a block: at most 256 x K0_LV_SPT each) */
+	uint32_t peak;
+};
+
+__device__ __forceinline__ void k0_level_add(k0_level_part &p, uint32_t fmt, int32_t vi, int32_t vq) {
+	const int32_t ci = vdl2_level_code(fmt, vi), cq = vdl2_level_code(fmt, vq);
+	p.si += ci; p.sq += cq;
+	p.pow += vdl2_level_pow(ci, cq);
+	p.nc += 1u | (vdl2_level_rail(fmt, vi) | vdl2_level_rail(fmt, vq)) << 16;
+	p.peak = max(p.peak, max(vdl2_level_mag(ci), vdl2_level_mag(cq)));
+}
+
+__device__ __forceinline__ k0_level_part k0_level_zero() { k0_level_part p; p.si = p.sq = 0; p.pow = 0; p.nc = 0; p.peak = 0; return p; }
+
+__device__ __forceinline__ k0_level_part k0_levels_warp(const k0_level_part &t) {
+	k0_level_part p;
+	p.si = __reduce_add_sync(0xFFFFFFFFu, t.si);
+	p.sq = __reduce_add_sync(0xFFFFFFFFu, t.sq);
+	p.pow = ((uint64_t)__reduce_add_sync(0xFFFFFFFFu, (uint32_t)(t.pow >> 16)) << 16) + __reduce_add_sync(0xFFFFFFFFu, (uint32_t)t.pow & 0xFFFFu);
+	p.nc = __reduce_add_sync(0xFFFFFFFFu, t.nc);
+	p.peak = __reduce_max_sync(0xFFFFFFFFu, t.peak);
+	return p;
+}
+
+__device__ __forceinline__ void k0_levels_commit(vdl2_levels *acc, const k0_level_part &p) {
+	const uint32_t n = p.nc & 0xFFFFu, clip = p.nc >> 16;
+	if(n == 0) return;
+	atomicAdd(reinterpret_cast<unsigned long long *>(&acc->samples), (unsigned long long)n);
+	if(p.si) atomicAdd(reinterpret_cast<unsigned long long *>(&acc->sum_i), (unsigned long long)(long long)p.si);
+	if(p.sq) atomicAdd(reinterpret_cast<unsigned long long *>(&acc->sum_q), (unsigned long long)(long long)p.sq);
+	if(p.pow) {
+		const uint64_t old = atomicAdd(reinterpret_cast<unsigned long long *>(&acc->pow_lo), (unsigned long long)p.pow);
+		if(vdl2_pow_carry(old, p.pow)) atomicAdd(reinterpret_cast<unsigned long long *>(&acc->pow_hi), 1ull);
+	}
+	if(clip) atomicAdd(reinterpret_cast<unsigned long long *>(&acc->clipped), (unsigned long long)clip);
+	if(p.peak) atomicMax(&acc->peak, p.peak);
+}
+
+/* the whole 256-thread block (every thread must call): the threads' sums t into acc */
+__device__ __forceinline__ void k0_levels_block(vdl2_levels *acc, const k0_level_part &t) {
+	__shared__ k0_level_part part[8];
+	const k0_level_part w = k0_levels_warp(t);
+	if((threadIdx.x & 31u) == 0) part[threadIdx.x >> 5] = w;
+	__syncthreads();
+	if(threadIdx.x == 0) {
+		k0_level_part b = part[0];
+		for(uint32_t k = 1; k < 8; k++) {
+			b.si += part[k].si; b.sq += part[k].sq; b.pow += part[k].pow; b.nc += part[k].nc; b.peak = max(b.peak, part[k].peak);
+		}
+		k0_levels_commit(acc, b);
+	}
+}
+
+template<bool LEVELS>
 __global__ void __launch_bounds__(256) k0_convert(const uint8_t *__restrict__ raw0, uint32_t n_pairs_p, uint32_t fmt,
 		const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t raw_stride, uint32_t out_stride,
-		const vdl2_chunk_args *__restrict__ ca) {
+		const vdl2_chunk_args *__restrict__ ca, vdl2_levels *__restrict__ lv) {
 	const uint32_t n_pairs = ca ? ca->n_pairs : n_pairs_p;
 	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + (size_t)blockIdx.y * raw_stride;   /* stream blockIdx.y */
 	float2 *out = out0 + (size_t)blockIdx.y * out_stride;
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if constexpr(!LEVELS) {
 	if(i >= n_pairs) return;
 	float re, im;
 	if(fmt == 0) {                                       /* src/demod.c:343-345, table from :349-354 */
@@ -63,14 +130,41 @@ __global__ void __launch_bounds__(256) k0_convert(const uint8_t *__restrict__ ra
 		im = __fdiv_rn((float)pl[n_pairs + i], 32768.0f);
 	}
 	out[i] = make_float2(re, im);
+	} else {
+		/* block b converts samples [b, b + 1) x 256 K0_LV_SPT, thread t those = t mod 256 */
+		if(blockIdx.x * 256u * K0_LV_SPT >= n_pairs) return;  /* (uniform over the block) */
+		k0_level_part t = k0_level_zero();
+#pragma unroll 4
+		for(uint32_t k = 0; k < K0_LV_SPT; k++) {
+			i = (blockIdx.x * K0_LV_SPT + k) * 256u + threadIdx.x;
+			if(i >= n_pairs) break;
+			int32_t vi, vq;
+			float re, im;
+			if(fmt == 0) {
+				uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
+				vi = v.x; vq = v.y;
+				re = __ldg(&levels[v.x]);
+				im = __ldg(&levels[v.y]);
+			} else {
+				if(fmt == 1) { short2 v = reinterpret_cast<const short2 *>(raw)[i]; vi = v.x; vq = v.y; }
+				else { const short *pl = reinterpret_cast<const short *>(raw); vi = pl[i]; vq = pl[n_pairs + i]; }
+				re = __fdiv_rn((float)vi, 32768.0f);
+				im = __fdiv_rn((float)vq, 32768.0f);
+			}
+			out[i] = make_float2(re, im);
+			k0_level_add(t, fmt, vi, vq);
+		}
+		k0_levels_block(lv + blockIdx.y, t);
+	}
 }
 
 /* K0 for the one-stream-per-channel layout: raw[s][i] -> out[i][s] float2 {re, im}, i.e. TIME-major across streams, so
  * that the 32 lanes of a K1 warp (32 different streams) read 256 contiguous bytes per sample.  32x32 tile through
  * shared memory: reads run along the samples of a stream, writes along the streams of a sample. */
+template<bool LEVELS>
 __global__ void __launch_bounds__(1024) k0_convert_lanes(const uint8_t *__restrict__ raw0, uint32_t n_pairs_p, uint32_t fmt,
 		const float *__restrict__ levels, float2 *__restrict__ out, uint32_t n_streams, uint32_t raw_stride, uint32_t out_stride,
-		uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *__restrict__ ca) {
+		uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *__restrict__ ca, vdl2_levels *__restrict__ lv) {
 	__shared__ float2 tile[32][33];
 	const uint32_t n_pairs = ca ? ca->n_pairs : n_pairs_p;
 	const uint8_t *raw = ca ? static_cast<const uint8_t *>(ca->raw) : raw0;
@@ -79,7 +173,7 @@ __global__ void __launch_bounds__(1024) k0_convert_lanes(const uint8_t *__restri
 	uint32_t s_in;                                    /* stream = channel that lives in column (slot) blockIdx.y * 32 + ty */
 	const bool have = vdl2_slot_channel(blockIdx.y * 32u + ty, lanes, full_warps, n_streams, s_in);
 	float re = 0.f, im = 0.f;
-	if(have && i_in < n_pairs) {
+	if(!LEVELS && have && i_in < n_pairs) {
 		const uint8_t *r = raw + (size_t)s_in * raw_stride;
 		if(fmt == 0) {
 			uchar2 v = reinterpret_cast<const uchar2 *>(r)[i_in];
@@ -89,10 +183,43 @@ __global__ void __launch_bounds__(1024) k0_convert_lanes(const uint8_t *__restri
 			re = __fdiv_rn((float)v.x, 32768.0f); im = __fdiv_rn((float)v.y, 32768.0f);
 		}
 	}
+	if constexpr(!LEVELS) {
 	tile[ty][tx] = make_float2(re, im);
 	__syncthreads();
 	const uint32_t i_out = blockIdx.x * 32u + ty, s_out = blockIdx.y * 32u + tx;
 	if(i_out < n_pairs && s_out < out_stride) out[(size_t)i_out * out_stride + s_out] = tile[tx][ty];
+	} else {
+		/* block b transposes the K0_LV_SPT tiles of samples [b, b + 1) x 32 K0_LV_SPT; warp ty sums stream s_in over all of
+		 * them and commits once */
+		k0_level_part t = k0_level_zero();
+		for(uint32_t k = 0; k < K0_LV_SPT; k++) {
+			const uint32_t i0 = (blockIdx.x * K0_LV_SPT + k) * 32u;
+			if(i0 >= n_pairs) break;                  /* (uniform over the block) */
+			const uint32_t j = i0 + tx;
+			re = im = 0.f;
+			if(have && j < n_pairs) {
+				const uint8_t *r = raw + (size_t)s_in * raw_stride;
+				int32_t vi, vq;
+				if(fmt == 0) {
+					uchar2 v = reinterpret_cast<const uchar2 *>(r)[j];
+					vi = v.x; vq = v.y;
+					re = __ldg(&levels[v.x]); im = __ldg(&levels[v.y]);
+				} else {
+					short2 v = reinterpret_cast<const short2 *>(r)[j];
+					vi = v.x; vq = v.y;
+					re = __fdiv_rn((float)v.x, 32768.0f); im = __fdiv_rn((float)v.y, 32768.0f);
+				}
+				k0_level_add(t, fmt, vi, vq);
+			}
+			if(k) __syncthreads();                        /* the previous tile has been written out */
+			tile[ty][tx] = make_float2(re, im);
+			__syncthreads();
+			const uint32_t i_out = i0 + ty, s_out = blockIdx.y * 32u + tx;
+			if(i_out < n_pairs && s_out < out_stride) out[(size_t)i_out * out_stride + s_out] = tile[tx][ty];
+		}
+		const k0_level_part p = k0_levels_warp(t);
+		if(have && tx == 0) k0_levels_commit(lv + s_in, p);
+	}
 }
 
 /* K0 for mixed-rate receivers: grid row r converts receiver r's n_dec x os_r samples, in its own format, from its own
@@ -116,42 +243,106 @@ __device__ __forceinline__ float2 k0_mixed_sample(const uint8_t *__restrict__ ra
 	return make_float2(re, im);
 }
 
+/* levels form of k0_mixed_sample: the raw values as well (the same loads and arithmetic) */
+__device__ __forceinline__ float2 k0_mixed_sample_raw(const uint8_t *__restrict__ raw, const vdl2_rx_input &in, uint32_t i,
+		const float *__restrict__ levels, int32_t &vi, int32_t &vq) {
+	if(in.fmt == 0) {
+		uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
+		vi = v.x; vq = v.y;
+		return make_float2(__ldg(&levels[v.x]), __ldg(&levels[v.y]));
+	}
+	short2 v;
+	if((reinterpret_cast<uintptr_t>(raw) & 3u) == 0) v = reinterpret_cast<const short2 *>(raw)[i];
+	else { const short *s = reinterpret_cast<const short *>(raw) + 2u * i; v = make_short2(s[0], s[1]); }
+	vi = v.x; vq = v.y;
+	return make_float2(__fdiv_rn((float)v.x, 32768.0f), __fdiv_rn((float)v.y, 32768.0f));
+}
+
+/* levels form of the per-receiver rows: block b of row r converts samples [b, b + 1) x 256 K0_LV_SPT of the row's n
+ * samples, sample i at byte offset at(i) of raw, into out[i], and counts them into acc */
+template<typename AT>
+__device__ __forceinline__ void k0_row_levels(const uint8_t *__restrict__ raw, const vdl2_rx_input &in, uint32_t n, AT at,
+		const float *__restrict__ levels, float2 *__restrict__ out, vdl2_levels *__restrict__ acc) {
+	k0_level_part t = k0_level_zero();
+#pragma unroll 4
+	for(uint32_t k = 0; k < K0_LV_SPT; k++) {
+		const uint32_t i = (blockIdx.x * K0_LV_SPT + k) * 256u + threadIdx.x;
+		if(i >= n) break;
+		int32_t vi, vq;
+		out[i] = k0_mixed_sample_raw(raw + at(i), in, 0, levels, vi, vq);
+		k0_level_add(t, in.fmt, vi, vq);
+	}
+	k0_levels_block(acc, t);
+}
+
+template<bool LEVELS>
 __global__ void __launch_bounds__(256) k0_convert_mixed(const uint8_t *__restrict__ raw0, uint32_t n_dec_p, const vdl2_rx_input *__restrict__ rx,
-		const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride, const vdl2_chunk_args *__restrict__ ca) {
+		const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride, const vdl2_chunk_args *__restrict__ ca,
+		vdl2_levels *__restrict__ lv) {
 	const uint32_t n_dec = ca ? ca->n_pairs : n_dec_p;
 	const vdl2_rx_input in = rx[blockIdx.y];
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if constexpr(!LEVELS) {
 	if(i >= n_dec * in.oversample) return;
 	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec);
 	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(raw, in, i, levels);
+	} else {
+		const uint32_t n = n_dec * in.oversample;
+		if(blockIdx.x * 256u * K0_LV_SPT >= n) return;      /* (uniform over the block) */
+		const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec);
+		const uint32_t bpp = in.fmt == 0 ? 2u : 4u;
+		k0_row_levels(raw, in, n, [bpp](uint32_t j) { return (size_t)j * bpp; }, levels, out0 + (size_t)blockIdx.y * out_stride, lv + blockIdx.y);
+	}
 }
 
 /* K0 on ragged spans: grid row r converts the span[r].n x os_r samples receiver r brought to this span, from its own place
  * in the span (its entry of the span's receiver table), into row r of the sample plane; rows past their count idle */
+template<bool LEVELS>
 __global__ void __launch_bounds__(256) k0_convert_ragged(const uint8_t *__restrict__ raw0, const vdl2_rx_input *__restrict__ rx,
 		const vdl2_rx_span *__restrict__ span, const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride,
-		const vdl2_chunk_args *__restrict__ ca) {
+		const vdl2_chunk_args *__restrict__ ca, vdl2_levels *__restrict__ lv) {
 	const vdl2_rx_input in = rx[blockIdx.y];
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if constexpr(!LEVELS) {
 	if(i >= span[blockIdx.y].n * in.oversample) return;
 	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + span[blockIdx.y].off;
 	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(raw, in, i, levels);
+	} else {
+		const uint32_t n = span[blockIdx.y].n * in.oversample;
+		if(blockIdx.x * 256u * K0_LV_SPT >= n) return;      /* (uniform over the block) */
+		const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + span[blockIdx.y].off;
+		const uint32_t bpp = in.fmt == 0 ? 2u : 4u;
+		k0_row_levels(raw, in, n, [bpp](uint32_t j) { return (size_t)j * bpp; }, levels, out0 + (size_t)blockIdx.y * out_stride, lv + blockIdx.y);
+	}
 }
 
 /* K0 on pushed spans: grid row r converts the span[r].n x os_r samples of receiver r where its pushes left them, in its
  * ring (ring[r]) from ring offset span[r].off on, wrapping at the ring's end, into row r of the sample plane.  The ring's
  * capacity is a multiple of the sample size and its tail advances in whole groups, so no sample straddles the wrap and
  * every cs16 sample starts 4-byte aligned. */
+template<bool LEVELS>
 __global__ void __launch_bounds__(256) k0_convert_rings(const uint8_t *__restrict__ rings, const vdl2_rx_input *__restrict__ rx,
 		const vdl2_rx_ring *__restrict__ ring, const vdl2_rx_span *__restrict__ span, const float *__restrict__ levels,
-		float2 *__restrict__ out0, uint32_t out_stride) {
+		float2 *__restrict__ out0, uint32_t out_stride, vdl2_levels *__restrict__ lv) {
 	const vdl2_rx_input in = rx[blockIdx.y];
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if constexpr(!LEVELS) {
 	if(i >= span[blockIdx.y].n * in.oversample) return;
 	const vdl2_rx_ring rg = ring[blockIdx.y];
 	uint64_t p = span[blockIdx.y].off + (uint64_t)i * (in.fmt == 0 ? 2u : 4u);     /* < 2 cap: a span is shorter than the ring */
 	if(p >= rg.cap) p -= rg.cap;
 	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(rings + rg.base + p, in, 0, levels);
+	} else {
+		const uint32_t n = span[blockIdx.y].n * in.oversample;
+		if(blockIdx.x * 256u * K0_LV_SPT >= n) return;      /* (uniform over the block) */
+		const vdl2_rx_ring rg = ring[blockIdx.y];
+		const uint64_t off = span[blockIdx.y].off, cap = rg.cap;
+		const uint32_t bpp = in.fmt == 0 ? 2u : 4u;
+		k0_row_levels(rings + rg.base, in, n, [off, cap, bpp](uint32_t j) {
+			uint64_t p = off + (uint64_t)j * bpp;               /* < 2 cap: a span is shorter than the ring */
+			return p >= cap ? p - cap : p;
+		}, levels, out0 + (size_t)blockIdx.y * out_stride, lv + blockIdx.y);
+	}
 }
 
 /* ------------------------------------------------------------------------------------------------
@@ -1460,8 +1651,10 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		vdl2_set_carveout(k1_mix_iir_decimate_packed<10, K1_BLOCK1, 10, true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_packed<10, K1_BLOCK1, 10, false>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_scalar<K1_BLOCK1>, pct);
-		vdl2_set_carveout(k0_convert, pct);
-		vdl2_set_carveout(k0_convert_lanes, pct);
+		vdl2_set_carveout(k0_convert<false>, pct);
+		vdl2_set_carveout(k0_convert<true>, pct);
+		vdl2_set_carveout(k0_convert_lanes<false>, pct);
+		vdl2_set_carveout(k0_convert_lanes<true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_lanes<20, true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_lanes<20, false>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_lanes<10, true>, pct);
@@ -1474,12 +1667,16 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		cudaFuncSetAttribute(k1_mix_iir_decimate_groups<OS, SYM>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_K1_SMEM_BUDGET); } while(0)
 		K1G_SETUP(20, true); K1G_SETUP(20, false); K1G_SETUP(10, true); K1G_SETUP(10, false); K1G_SETUP(13, true); K1G_SETUP(13, false);
 #undef K1G_SETUP
-		vdl2_set_carveout(k0_convert_mixed, pct);
+		vdl2_set_carveout(k0_convert_mixed<false>, pct);
+		vdl2_set_carveout(k0_convert_mixed<true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_mixed<true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_mixed<false>, pct);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_mixed<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_mixed<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
-		vdl2_set_carveout(k0_convert_ragged, pct);
+		vdl2_set_carveout(k0_convert_ragged<false>, pct);
+		vdl2_set_carveout(k0_convert_ragged<true>, pct);
+		vdl2_set_carveout(k0_convert_rings<false>, pct);
+		vdl2_set_carveout(k0_convert_rings<true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_ragged<true>, pct);
 		vdl2_set_carveout(k1_mix_iir_decimate_ragged<false>, pct);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_ragged<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
@@ -1508,42 +1705,52 @@ extern "C" int vdl2_kernels_init_device(int device) {
 }
 
 extern "C" int vdl2_launch_k0(const void *raw, uint32_t n_pairs, uint32_t fmt, const float *levels, float *out2, uint32_t n_streams,
-		uint32_t raw_stride, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st) {
+		uint32_t raw_stride, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st) {
 	if(n_pairs == 0 || n_streams == 0) return 0;
-	k0_convert<<<dim3((n_pairs + 255) / 256, n_streams), 256, 0, st>>>(static_cast<const uint8_t *>(raw), n_pairs, fmt, levels,
-			reinterpret_cast<float2 *>(out2), raw_stride, out_stride, ca);
+	const uint32_t per_block = lv ? 256u * K0_LV_SPT : 256u;
+	auto k = lv ? k0_convert<true> : k0_convert<false>;
+	k<<<dim3((n_pairs + per_block - 1) / per_block, n_streams), 256, 0, st>>>(static_cast<const uint8_t *>(raw), n_pairs, fmt, levels,
+			reinterpret_cast<float2 *>(out2), raw_stride, out_stride, ca, lv);
 	return (int)cudaGetLastError();
 }
 
 extern "C" int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t fmt, const float *levels, float *out2, uint32_t n_streams,
-		uint32_t raw_stride, uint32_t out_stride, uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *ca, cudaStream_t st) {
+		uint32_t raw_stride, uint32_t out_stride, uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st) {
 	if(n_pairs == 0 || n_streams == 0) return 0;
-	k0_convert_lanes<<<dim3((n_pairs + 31) / 32, (out_stride + 31) / 32), dim3(32, 32), 0, st>>>(static_cast<const uint8_t *>(raw), n_pairs, fmt,
-			levels, reinterpret_cast<float2 *>(out2), n_streams, raw_stride, out_stride, lanes, full_warps, ca);
+	const uint32_t per_block = lv ? 32u * K0_LV_SPT : 32u;
+	auto k = lv ? k0_convert_lanes<true> : k0_convert_lanes<false>;
+	k<<<dim3((n_pairs + per_block - 1) / per_block, (out_stride + 31) / 32), dim3(32, 32), 0, st>>>(static_cast<const uint8_t *>(raw), n_pairs, fmt,
+			levels, reinterpret_cast<float2 *>(out2), n_streams, raw_stride, out_stride, lanes, full_warps, ca, lv);
 	return (int)cudaGetLastError();
 }
 
 extern "C" int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *rx, uint32_t n_rx, uint32_t os_max, const float *levels,
-		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st) {
+		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st) {
 	if(n_dec == 0 || n_rx == 0) return 0;
-	k0_convert_mixed<<<dim3((n_dec * os_max + 255) / 256, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), n_dec, rx, levels,
-			reinterpret_cast<float2 *>(out2), out_stride, ca);
+	const uint32_t per_block = lv ? 256u * K0_LV_SPT : 256u;
+	auto k = lv ? k0_convert_mixed<true> : k0_convert_mixed<false>;
+	k<<<dim3((n_dec * os_max + per_block - 1) / per_block, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), n_dec, rx, levels,
+			reinterpret_cast<float2 *>(out2), out_stride, ca, lv);
 	return (int)cudaGetLastError();
 }
 
 extern "C" int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
-		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st) {
+		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st) {
 	if(width == 0 || n_rx == 0) return 0;
-	k0_convert_ragged<<<dim3((width * os_max + 255) / 256, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), rx, span, levels,
-			reinterpret_cast<float2 *>(out2), out_stride, ca);
+	const uint32_t per_block = lv ? 256u * K0_LV_SPT : 256u;
+	auto k = lv ? k0_convert_ragged<true> : k0_convert_ragged<false>;
+	k<<<dim3((width * os_max + per_block - 1) / per_block, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), rx, span, levels,
+			reinterpret_cast<float2 *>(out2), out_stride, ca, lv);
 	return (int)cudaGetLastError();
 }
 
 extern "C" int vdl2_launch_k0_rings(const uint8_t *rings, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_ring *ring, const vdl2_rx_span *span,
-		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, cudaStream_t st) {
+		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, vdl2_levels *lv, cudaStream_t st) {
 	if(width == 0 || n_rx == 0) return 0;
-	k0_convert_rings<<<dim3((width * os_max + 255) / 256, n_rx), 256, 0, st>>>(rings, rx, ring, span, levels,
-			reinterpret_cast<float2 *>(out2), out_stride);
+	const uint32_t per_block = lv ? 256u * K0_LV_SPT : 256u;
+	auto k = lv ? k0_convert_rings<true> : k0_convert_rings<false>;
+	k<<<dim3((width * os_max + per_block - 1) / per_block, n_rx), 256, 0, st>>>(rings, rx, ring, span, levels,
+			reinterpret_cast<float2 *>(out2), out_stride, lv);
 	return (int)cudaGetLastError();
 }
 

@@ -154,24 +154,26 @@ extern "C" {
 #endif
 /* once per device (thread-safe): the shared-memory carve-out every kernel of the chain asks for */
 int vdl2_kernels_init_device(int device);
+/* Every K0 launcher takes lv: NULL, or the per-input accumulators (vdl2_levels, one per stream or receiver) that the levels
+ * form of the kernel adds the chunk's samples to (VDL2GPU_FLAG_INPUT_LEVELS) */
 /* n_streams streams of n_pairs samples each: raw stream s at raw + s * raw_stride bytes, output at out2 + s * out_stride float2 */
 int vdl2_launch_k0(const void *raw, uint32_t n_pairs, uint32_t fmt, const float *levels, float *out2, uint32_t n_streams,
-		uint32_t raw_stride, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
+		uint32_t raw_stride, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
 /* one stream per channel: raw[s][i] -> out2[i][out_stride] float2, time-major across streams */
 int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t fmt, const float *levels, float *out2, uint32_t n_streams,
-		uint32_t raw_stride, uint32_t out_stride, uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *ca, cudaStream_t st);
+		uint32_t raw_stride, uint32_t out_stride, uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
 /* mixed-rate receivers: row r converts n_dec x rx[r].oversample samples in format rx[r].fmt from raw + n_dec x
  * rx[r].off_per_dec into out2 + r x out_stride float2 (n_dec from ca->n_pairs when ca is given) */
 int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *rx, uint32_t n_rx, uint32_t os_max, const float *levels,
-		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
+		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
 /* ragged spans: row r converts span[r].n x rx[r].oversample samples from raw + span[r].off; width = the largest span[r].n
  * (sizes the grid) */
 int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
-		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, cudaStream_t st);
+		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
 /* pushed spans: row r converts span[r].n x rx[r].oversample samples from receiver r's ring (rings + ring[r].base), starting
  * at ring offset span[r].off and wrapping at ring[r].cap; width = the largest span[r].n (sizes the grid) */
 int vdl2_launch_k0_rings(const uint8_t *rings, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_ring *ring, const vdl2_rx_span *span,
-		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, cudaStream_t st);
+		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, vdl2_levels *lv, cudaStream_t st);
 int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st);
 int vdl2_launch_copy_hist(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k2a(const vdl2_k2_params *p, cudaStream_t st);

@@ -52,8 +52,9 @@ enum {
 	VDL2GPU_FLAG_K1_SCALAR = 1u << 2,    /* use the plain per-sample K1 kernel instead of the pipelined one */
 	VDL2GPU_FLAG_NO_OVERLAP = 1u << 3,   /* one stream: do not run K0/K1 of chunk c+1 beside K2/K3 of chunk c (profiling) */
 	VDL2GPU_FLAG_NO_GRAPH = 1u << 4,     /* launch every kernel individually instead of replaying the per-chunk CUDA graphs */
-	VDL2GPU_FLAG_RAGGED = 1u << 5        /* vdl2gpu_create_mixed_receivers only: every receiver brings its own number of decimated
+	VDL2GPU_FLAG_RAGGED = 1u << 5,       /* vdl2gpu_create_mixed_receivers only: every receiver brings its own number of decimated
 	                                      * samples to a span (vdl2gpu_submit_ragged); every other create function refuses it */
+	VDL2GPU_FLAG_INPUT_LEVELS = 1u << 6  /* measure every input's levels on the device (vdl2gpu_get_input_levels); any create function */
 };
 
 typedef struct {
@@ -323,6 +324,38 @@ int vdl2gpu_get_stats(vdl2gpu_ctx *ctx, vdl2gpu_stats *out);
 /* per-channel counters, 9 x uint64 per channel in the order: sync_good, hdr_crc_good, bursts, burst_err,
  * blocks_processed, blocks_fec_ok, msg_good, fcs_good, fcs_bad.  Implies a flush of device work. */
 int vdl2gpu_get_channel_counters(vdl2gpu_ctx *ctx, uint64_t *out, uint32_t n_channels);
+
+/* Input levels (VDL2GPU_FLAG_INPUT_LEVELS): exact integer figures of every raw sample an input has brought, for telling a
+ * dead or disconnected receiver, a gain set too high or a DC spike from a quiet sky without waiting for traffic.  A
+ * component's integer code c is, for cu8, c = 2v - 255 (c / 255 is exactly the reference's (v - 127.5) / 127.5,
+ * src/demod.c:349-354) and, for cs16, c = v (c / 32768, src/demod.c:361-363).  A sample is clipped when its I or Q sits on
+ * a rail: cu8 v = 0 or 255, cs16 v = -32768 or 32767.  Mean power in dBFS is 10 log10(pow / (samples x full_scale^2)),
+ * with pow = pow_hi x 2^64 + pow_lo; the DC offsets are sum_i / (samples x full_scale) and sum_q / (samples x full_scale). */
+typedef struct {
+	uint64_t samples;            /* complex samples measured */
+	int64_t sum_i, sum_q;        /* sum of c over the I and over the Q components */
+	uint64_t pow_lo, pow_hi;     /* sum of (c_I^2 + c_Q^2), one unsigned 128-bit integer */
+	uint64_t clipped;            /* complex samples with I or Q on a rail */
+	uint32_t peak;               /* largest |c| of any component */
+	uint32_t full_scale;         /* 255 (cu8) or 32768 (cs16) */
+} vdl2gpu_input_levels;          /* 56 bytes */
+/* out[k] = the levels of input k for k < n.  Inputs: a fan-out context has one, an n_streams context n_streams, a
+ * receivers context (vdl2gpu_create_receivers, vdl2gpu_create_mixed_receivers) one per receiver, in receiver order.
+ *   - Cumulative from create (for a receiver added by vdl2gpu_update_receivers: from when it joined), over every sample of
+ *     every chunk or span submitted before the call; the call waits for that work, as vdl2gpu_get_channel_counters does.
+ *     Host, device and planar submits count alike.
+ *   - Pushed input counts once it enters a span: positions[r] x oversample_r complex samples for receiver r.  Bytes still
+ *     queued, and bytes a restart drops, are not counted.  vdl2gpu_restart_receiver keeps counting, as the per-channel
+ *     counters do.  vdl2gpu_update_receivers: a kept receiver carries its levels to its new index, a new receiver starts
+ *     at zero, a removed receiver's levels are gone.
+ *   - The integers are exact and do not depend on how the stream was cut (chunk, span and push lengths, ragged counts),
+ *     n_inflight, graphs or trace.  The sum of squares never wraps.
+ *   - Frames, metadata, counters, trace events and vdl2gpu_stats are the same with the flag on or off.  A context without
+ *     the flag allocates and launches nothing for it.
+ * Runs on the control thread, concurrently with vdl2gpu_push (which does not touch the figures).  VDL2GPU_EINVAL (with
+ * vdl2gpu_last_error) for a NULL context or output, n larger than the number of inputs, or a context created without
+ * VDL2GPU_FLAG_INPUT_LEVELS.  Not available through the stage stubs or the drop-in symbols. */
+int vdl2gpu_get_input_levels(vdl2gpu_ctx *ctx, vdl2gpu_input_levels *out, uint32_t n);
 
 /* ---- multi-GPU ingest (one process per GPU; global channel k is demodulated on GPU k mod N, the reference's
  * channel threads share nothing but the read-only sample buffer: src/dumpvdl2.c:117-135, src/demod.c:50,300-301).
