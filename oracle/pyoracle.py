@@ -73,6 +73,14 @@ def lib():
     L.vo_dec_tap.argtypes = [C.c_void_p]
     L.vo_counters.restype = C.POINTER(C.c_uint64)
     L.vo_counters.argtypes = [C.c_void_p]
+    L.vo_process_dec.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.vo_enable_state_tap.argtypes = [C.c_void_p, C.c_int]
+    L.vo_state_count.restype = C.c_uint64
+    L.vo_state_count.argtypes = [C.c_void_p]
+    L.vo_state_tap.restype = C.POINTER(C.c_uint32)
+    L.vo_state_tap.argtypes = [C.c_void_p]
+    L.vo_pherr1_tap.restype = C.POINTER(C.c_float)
+    L.vo_pherr1_tap.argtypes = [C.c_void_p]
     L.vo_levels_u8.argtypes = [C.c_void_p]
     L.vo_sincos_lut.argtypes = [C.c_void_p, C.c_void_p]
     L.vo_lpf_design.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p]
@@ -119,7 +127,7 @@ class Frame:
 class Oracle:
     """Whole-path oracle for one IQ stream fanned out to n channels."""
 
-    def __init__(self, sample_rate, oversample, fmt, centerfreq, freqs, max_ppm=0.0, trace=False, dec_tap=False):
+    def __init__(self, sample_rate, oversample, fmt, centerfreq, freqs, max_ppm=0.0, trace=False, dec_tap=False, state_tap=False):
         self.L = lib()
         self.freqs = np.ascontiguousarray(freqs, dtype=np.uint32)
         self.n_channels = len(self.freqs)
@@ -130,6 +138,8 @@ class Oracle:
             self.L.vo_enable_trace(self.h, 1)
         if dec_tap:
             self.L.vo_enable_dec_tap(self.h, 1)
+        if state_tap:
+            self.L.vo_enable_state_tap(self.h, 1)
 
     def close(self):
         if self.h:
@@ -151,6 +161,12 @@ class Oracle:
         for off in range(0, b.size, chunk_bytes):
             part = b[off:off + chunk_bytes]
             self.L.vo_process(self.h, part.ctypes.data, part.size)
+
+    def process_dec(self, dec):
+        """demod() of every channel on decimated samples [n_dec][n_channels][2] (float32), the front end skipped"""
+        d = np.ascontiguousarray(dec, np.float32)
+        assert d.ndim == 3 and d.shape[1:] == (self.n_channels, 2)
+        self.L.vo_process_dec(self.h, d.ctypes.data, d.shape[0])
 
     def frames(self):
         n = self.L.vo_num_frames(self.h)
@@ -183,6 +199,20 @@ class Oracle:
             return np.zeros((0, self.n_channels, 2), np.float32)
         p = self.L.vo_dec_tap(self.h)
         return np.ctypeslib.as_array(p, shape=(n, self.n_channels, 2)).copy()
+
+    def states(self):
+        """the state each decimated sample of process_dec met, [n][n_channels] uint32 (layout: vo_enable_state_tap)"""
+        n = self.L.vo_state_count(self.h)
+        if n == 0:
+            return np.zeros((0, self.n_channels), np.uint32)
+        return np.ctypeslib.as_array(self.L.vo_state_tap(self.h), shape=(n, self.n_channels)).copy()
+
+    def pherr1(self):
+        """the sync metric of the previous attempt (pherr[1]) each decimated sample of process_dec met, [n][n_channels]"""
+        n = self.L.vo_state_count(self.h)
+        if n == 0:
+            return np.zeros((0, self.n_channels), np.float32)
+        return np.ctypeslib.as_array(self.L.vo_pherr1_tap(self.h), shape=(n, self.n_channels)).copy()
 
     def counters(self):
         p = self.L.vo_counters(self.h)
@@ -277,3 +307,26 @@ def run_ref(path, fmt, oversample, centerfreq, freqs, flavour="strict", chunk=No
         elif line.startswith("STATS"):
             stats = {k: float(v) for k, v in kv.items()}
     return frames, stats
+
+
+def run_ref_dec(dec, freqs, max_ppm=0.0):
+    """the reference's own demod() (oracle/_ref/vdl2_ref_dec) on decimated samples [n][channels][2]: its FRAME lines"""
+    import tempfile
+    exe = os.path.join(_HERE, "_ref", "vdl2_ref_dec")
+    if not os.path.exists(exe):
+        raise FileNotFoundError("oracle/_ref not built")
+    with tempfile.NamedTemporaryFile(suffix=".f32") as tf:
+        tf.write(np.ascontiguousarray(dec, np.float32).tobytes())
+        tf.flush()
+        cmd = [exe, "--freqs", ",".join(str(int(f)) for f in freqs)]
+        if max_ppm:
+            cmd += ["--max-ppm", str(max_ppm)]
+        out = subprocess.run(cmd + [tf.name], check=True, capture_output=True, text=True).stdout
+    return [l for l in out.splitlines() if l.startswith("FRAME")]
+
+
+def frame_line(f):
+    """a Frame in the reference harness's FRAME line format (oracle/ref_harness.c)"""
+    return (f"FRAME ch={f.channel} freq={f.freq} idx={f.idx} len={len(f.data)} synd={f.synd_weight} datalen={f.datalen_octets} "
+            f"fec={f.num_fec_corrections} pwr={float(np.float32(f.frame_pwr_dbfs)):.9g} nf={float(np.float32(f.nf_pwr_dbfs)):.9g} "
+            f"ppm={float(np.float32(f.ppm_error)):.9g} hex={f.data.hex()}")

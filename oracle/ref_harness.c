@@ -140,12 +140,29 @@ static void *chan_thread(void *arg) {
 	return process_samples(a->v);   /* never returns */
 }
 
+/* one FRAME line per captured frame, by channel in push order; returns the number of frames */
+static size_t print_captures(void) {
+	size_t nframes = 0;
+	for(int i = 0; i < num_channels; i++) {
+		nframes += captures[i].count;
+		for(captured_t *c = captures[i].head; c; c = c->next) {
+			printf("FRAME ch=%d freq=%u idx=%d len=%zu synd=%u datalen=%u fec=%d pwr=%.9g nf=%.9g ppm=%.9g hex=",
+					i, c->md.freq, c->md.idx, c->len, c->md.synd_weight, c->md.datalen_octets,
+					c->md.num_fec_corrections, c->md.frame_pwr_dbfs, c->md.nf_pwr_dbfs, c->md.ppm_error);
+			for(size_t k = 0; k < c->len; k++) printf("%02x", c->buf[k]);
+			printf("\n");
+		}
+	}
+	return nframes;
+}
+
 static double now_s(void) {
 	struct timespec ts;
 	clock_gettime(CLOCK_MONOTONIC, &ts);
 	return ts.tv_sec + 1e-9 * ts.tv_nsec;
 }
 
+#ifndef REF_HARNESS_NO_MAIN
 int main(int argc, char **argv) {
 	char const *fmt = "u8", *freqs_s = NULL, *file = NULL;
 	uint32_t oversample = 10, centerfreq = 0, chunk = FILE_BUFSIZE;
@@ -255,17 +272,7 @@ int main(int argc, char **argv) {
 	pthread_barrier_wait(&demods_ready);     /* drain: reference src/dumpvdl2.c:1170 */
 	double t1 = now_s();
 
-	size_t nframes = 0;
-	for(int i = 0; i < num_channels; i++) {
-		nframes += captures[i].count;
-		for(captured_t *c = captures[i].head; c; c = c->next) {
-			printf("FRAME ch=%d freq=%u idx=%d len=%zu synd=%u datalen=%u fec=%d pwr=%.9g nf=%.9g ppm=%.9g hex=",
-					i, c->md.freq, c->md.idx, c->len, c->md.synd_weight, c->md.datalen_octets,
-					c->md.num_fec_corrections, c->md.frame_pwr_dbfs, c->md.nf_pwr_dbfs, c->md.ppm_error);
-			for(size_t k = 0; k < c->len; k++) printf("%02x", c->buf[k]);
-			printf("\n");
-		}
-	}
+	size_t nframes = print_captures();
 	uint64_t iq_samples = total_bytes / (is_s16 ? 4 : 2);
 	printf("STATS channels=%d iq_samples=%llu frames=%zu wall_s=%.6f ch_msamples_per_s=%.3f\n",
 			num_channels, (unsigned long long)iq_samples, nframes, t1 - t0,
@@ -273,3 +280,4 @@ int main(int argc, char **argv) {
 	fflush(stdout);
 	_exit(0);   /* channel threads are parked on the barrier; no join (same as the reference's shutdown) */
 }
+#endif

@@ -503,6 +503,7 @@ struct vo_ctx {
 	uint8_t *arena; uint32_t arena_used, arena_cap;
 	int trace; vo_event *events; uint32_t n_events, cap_events;
 	int tap; float *dec; uint64_t dec_count, dec_cap;
+	int state_tap; uint32_t *state; float *pherr1; uint64_t state_count, state_cap;
 	uint64_t *counters;
 };
 
@@ -769,7 +770,7 @@ vo_ctx *vo_create(uint32_t sample_rate, uint32_t oversample, int fmt, uint32_t c
 void vo_destroy(vo_ctx *c) {
 	if(!c) return;
 	for(uint32_t k = 0; k < c->n_channels; k++) free(c->ch[k].bits);
-	free(c->ch); free(c->sbuf); free(c->frames); free(c->arena); free(c->events); free(c->dec); free(c->counters);
+	free(c->ch); free(c->sbuf); free(c->frames); free(c->arena); free(c->events); free(c->dec); free(c->state); free(c->pherr1); free(c->counters);
 	free(c);
 }
 
@@ -835,6 +836,39 @@ void vo_process(vo_ctx *c, const uint8_t *buf, uint32_t len) {
 	if(c->tap) c->dec_count += dec_new;
 }
 
+/* the demodulator state a decimated sample meets, packed for vo_state_tap (layout in vdl2_oracle.h) */
+static uint32_t pack_state(const chan_t *v) {
+	return (uint32_t)v->ring_pos | ((uint32_t)(uint8_t)(int8_t)v->sclk << 8) | ((uint32_t)(v->demod_state == ST_LOCKED) << 16)
+		| ((uint32_t)(v->decoder_state == DS_IDLE) << 17) | ((uint32_t)v->nfcnt << 18);
+}
+
+/* demod() of every channel on decimated samples: the sample loop of process_samples (src/demod.c:302-329) after
+ * the decimation, without the front end */
+void vo_process_dec(vo_ctx *c, const float *dec, uint32_t n_dec) {
+	if(n_dec == 0) return;
+	if(c->state_tap) {
+		uint64_t need = (c->state_count + n_dec) * c->n_channels;
+		if(need > c->state_cap) {
+			c->state_cap = 2 * need + 1024;
+			c->state = realloc(c->state, c->state_cap * sizeof(uint32_t));
+			c->pherr1 = realloc(c->pherr1, c->state_cap * sizeof(float));
+		}
+	}
+	for(uint32_t k = 0; k < c->n_channels; k++) {
+		chan_t *v = &c->ch[k];
+		for(uint32_t n = 0; n < n_dec; n++) {
+			const float *d = &dec[((size_t)n * c->n_channels + k) * 2];
+			if(c->state_tap) {
+				c->state[(c->state_count + n) * c->n_channels + k] = pack_state(v);
+				c->pherr1[(c->state_count + n) * c->n_channels + k] = v->pherr[1];
+			}
+			demod_step(c, v, k, d[0], d[1]);
+			v->dec_index++;
+		}
+	}
+	if(c->state_tap) c->state_count += n_dec;
+}
+
 uint32_t vo_num_frames(const vo_ctx *c) { return c->n_frames; }
 const vo_frame *vo_frames(const vo_ctx *c) { return c->frames; }
 const uint8_t *vo_frame_bytes(const vo_ctx *c) { return c->arena; }
@@ -845,3 +879,7 @@ void vo_enable_dec_tap(vo_ctx *c, int on) { c->tap = on; }
 uint64_t vo_dec_count(const vo_ctx *c) { return c->dec_count; }
 const float *vo_dec_tap(const vo_ctx *c) { return c->dec; }
 const uint64_t *vo_counters(const vo_ctx *c) { return c->counters; }
+void vo_enable_state_tap(vo_ctx *c, int on) { c->state_tap = on; }
+uint64_t vo_state_count(const vo_ctx *c) { return c->state_count; }
+const uint32_t *vo_state_tap(const vo_ctx *c) { return c->state; }
+const float *vo_pherr1_tap(const vo_ctx *c) { return c->pherr1; }

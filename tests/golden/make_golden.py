@@ -48,9 +48,31 @@ def reference_checks(ref_dir):
     print("reference_checks: " + ", ".join(f"{k} {len(v['frames'])} frames" for k, v in out.items() if "frames" in v))
 
 
+def k2_corpus_reference():
+    """the reference's own demod() on the decimated samples of the K2 corpus (tests/k2_corpus.py): per channel, the
+    number of frames and a digest of their FRAME lines (strict build, oracle/ref_dec_harness.c), on the channels where
+    the reference's behaviour is defined"""
+    import hashlib
+    from tests import k2_corpus as kc
+    out = {}
+    for name in kc.STAGES:
+        s, ok = kc.stage(name), set(kc.reference_defined(name))
+        per = {}
+        for line in po.run_ref_dec(s["dec"], s["freqs"], s["max_ppm"]):
+            if int(line.split()[1][3:]) in ok:
+                per.setdefault(int(line.split()[1][3:]), []).append(line)
+        out[name] = dict(dec_sha256=hashlib.sha256(s["dec"].tobytes()).hexdigest(), max_ppm=s["max_ppm"],
+                         n_frames=sum(len(v) for v in per.values()),
+                         channels={str(c): [len(v), hashlib.sha256("\n".join(v).encode()).hexdigest()[:16]] for c, v in sorted(per.items())})
+    with open(os.path.join(cases.GOLDEN, "k2_corpus_reference.json"), "w") as f:
+        json.dump(out, f, indent=0)
+    print("k2_corpus_reference: " + ", ".join(f"{k} {v['n_frames']} frames" for k, v in out.items()))
+
+
 def main(ref_dir):
     po.build()
     reference_checks(ref_dir)
+    k2_corpus_reference()
     for name, fn in cases.ALL_GOLDEN.items():
         c = fn()
         with tempfile.NamedTemporaryFile(suffix=".iq", delete=False) as tf:

@@ -94,7 +94,8 @@ int hostsim_k1(const float *samples /*[n][2]*/, uint32_t n_pairs, uint32_t rate,
 int hostsim_k2k3(const float *dec /*[n_dec][n_ch][2]*/, uint32_t n_dec, uint32_t n_ch, const uint32_t *freqs,
 		uint32_t rate, float max_ppm, uint8_t *out, uint32_t out_cap, uint32_t *out_used, uint32_t *n_records,
 		vdl2_event_rec *events, uint32_t event_cap, uint32_t *n_events, uint32_t *chan_counters /*[n_ch][2]: sync, hdr_good*/,
-		int use_pre /* 1: consume the parallel pre-pass like K2 does; 0: always evaluate from the ring */) {
+		int use_pre /* 1: consume the parallel pre-pass like K2 does; 0: always evaluate from the ring */,
+		const uint32_t *launches /* launch lengths in decimated samples, repeated; nullptr: 1024 */, uint32_t n_launches) {
 	host_tables *h = new host_tables();
 	make_tables(*h, rate);
 	const uint32_t n_slots = 3 * n_ch + 16;
@@ -114,8 +115,8 @@ int hostsim_k2k3(const float *dec /*[n_dec][n_ch][2]*/, uint32_t n_dec, uint32_t
 	for(uint32_t ch = 0; ch < n_ch; ch++) vdl2_chan_init(chans[ch], freqs[ch]);
 	*out_used = 0; *n_records = 0;
 	vdl2_burst_work *w = new vdl2_burst_work();
-	/* the kernels process chunk by chunk: K2 over all channels, then K3 over the ready list; mimic with
-	 * chunks of 1024 decimated samples so that slot recycling is exercised */
+	/* the kernels process launch by launch: K2 over all channels, then K3 over the ready list.  Every launch restarts
+	 * the walk with the channel state carried over, as K2 does, so each one ends in its own walk tail. */
 	/* K2a emulation: phase plane with a 160-row zero history, magnitude plane */
 	std::vector<float> phase((size_t)(n_dec + VDL2_SYNC_BUFLEN) * n_ch, 0.f), mag((size_t)n_dec * n_ch);
 	for(uint32_t m = 0; m < n_dec; m++)
@@ -125,8 +126,9 @@ int hostsim_k2k3(const float *dec /*[n_dec][n_ch][2]*/, uint32_t n_dec, uint32_t
 			mag[(size_t)m * n_ch + ch] = vdl2_mag_of(d[0], d[1]);
 		}
 	const float2x *dec2 = reinterpret_cast<const float2x *>(dec);
-	for(uint32_t base = 0; base < n_dec; base += 1024) {
-		uint32_t n = n_dec - base < 1024 ? n_dec - base : 1024;
+	for(uint32_t base = 0, li = 0; base < n_dec; li++) {
+		const uint32_t len = launches && n_launches ? launches[li % n_launches] : 1024u;
+		uint32_t n = n_dec - base < len ? n_dec - base : len;
 		for(uint32_t ch = 0; ch < n_ch; ch++) {
 			uint32_t m = 0;
 			if(use_pre == 4) {                /* the kernel's staged ring walk (MODE 3): same control flow, the cp.async copies done at once */
@@ -238,6 +240,7 @@ int hostsim_k2k3(const float *dec /*[n_dec][n_ch][2]*/, uint32_t n_dec, uint32_t
 			free_list[ctl.free_top++] = (int32_t)ready[b];
 		}
 		ctl.n_ready = 0;
+		base += n;
 	}
 	for(uint32_t ch = 0; ch < n_ch; ch++) { chan_counters[2 * ch] = chans[ch].cnt_sync; chan_counters[2 * ch + 1] = chans[ch].cnt_hdr_good; }
 	*n_events = ctl.n_events < event_cap ? ctl.n_events : event_cap;

@@ -72,20 +72,24 @@ def k1(samples, rate, oversample, centerfreq, freqs):
     return dec
 
 
-def k2k3(dec, freqs, rate, max_ppm=0.0, trace=True, use_pre=True):
+def k2k3(dec, freqs, rate, max_ppm=0.0, trace=True, use_pre=True, launches=None, event_cap=1 << 16):
+    """K2 + K3 over a whole decimated stream, fed in launches of the given lengths (repeated; default 1024)"""
     d = np.ascontiguousarray(dec, np.float32)
+    sched = np.ascontiguousarray(launches if launches is not None else [], np.uint32)
     f = np.ascontiguousarray(freqs, np.uint32)
     n_dec, n_ch = d.shape[0], d.shape[1]
     out = np.zeros(8 << 20, np.uint8)
     used, nrec, nev = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
-    cap = 1 << 16
+    cap = event_cap
     ev = (Ev * cap)()
     cnt = np.zeros((n_ch, 2), np.uint32)
     rc = lib().hostsim_k2k3(d.ctypes.data_as(C.c_void_p), C.c_uint32(n_dec), C.c_uint32(n_ch), f.ctypes.data_as(C.c_void_p),
                             C.c_uint32(rate), C.c_float(max_ppm), out.ctypes.data_as(C.c_void_p), C.c_uint32(out.size),
                             C.byref(used), C.byref(nrec), C.cast(ev, C.c_void_p) if trace else None, C.c_uint32(cap), C.byref(nev),
-                            cnt.ctypes.data_as(C.c_void_p), C.c_int(int(use_pre)))       # 0 per-sample, 1 blocked, 2 blocked + unwrap table, 3 ring walk
+                            cnt.ctypes.data_as(C.c_void_p), C.c_int(int(use_pre)),      # 0 per-sample, 1 blocked, 2 blocked + unwrap table, 3 ring walk
+                            sched.ctypes.data_as(C.c_void_p) if sched.size else None, C.c_uint32(sched.size))
     assert rc == 0, f"hostsim pool overflow / error {rc}"
+    assert nev.value < cap, "hostsim event buffer full"
     recs = parse_records(out, used.value)
     events = [dict(channel=ev[k].channel, kind=ev[k].kind, dec_index=ev[k].dec_index, i=list(ev[k].i),
                    f=np.array(list(ev[k].f), np.float32)) for k in range(nev.value)]
