@@ -16,6 +16,8 @@ LIB_PATH = os.path.join(_HERE, "libvdl2gpu.so")
 FMT_U8, FMT_S16 = 0, 1
 FLAG_TRACE, FLAG_KEEP_DEC, FLAG_K1_SCALAR, FLAG_NO_OVERLAP, FLAG_NO_GRAPH, FLAG_RAGGED = 1, 2, 4, 8, 16, 32
 FLAG_INPUT_LEVELS = 64
+FLAG_CHANNEL_LEVELS = 128
+CHANNEL_LEVEL_BINS = 40
 NUM_COUNTERS = 9
 COUNTER_NAMES = ["sync_good", "hdr_crc_good", "bursts", "burst_err", "blocks_processed",
                  "blocks_fec_ok", "msg_good", "fcs_good", "fcs_bad"]
@@ -63,6 +65,11 @@ class _Stats(C.Structure):
 class _InputLevels(C.Structure):
     _fields_ = [("samples", C.c_uint64), ("sum_i", C.c_int64), ("sum_q", C.c_int64), ("pow_lo", C.c_uint64),
                 ("pow_hi", C.c_uint64), ("clipped", C.c_uint64), ("peak", C.c_uint32), ("full_scale", C.c_uint32)]
+
+
+class _ChannelLevels(C.Structure):
+    _fields_ = [("hist", C.c_uint64 * CHANNEL_LEVEL_BINS), ("pow_lo", C.c_uint64), ("pow_hi", C.c_uint64), ("peak_pow", C.c_float),
+                ("mag_lp", C.c_float), ("mag_nf", C.c_float), ("nf_pwr_dbfs", C.c_float)]
 
 
 class _Event(C.Structure):
@@ -113,6 +120,7 @@ def load_library():
     L.vdl2gpu_get_stats.argtypes = [C.c_void_p, C.POINTER(_Stats)]
     L.vdl2gpu_get_channel_counters.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_get_input_levels.argtypes = [C.c_void_p, C.POINTER(_InputLevels), C.c_uint32]
+    L.vdl2gpu_get_channel_levels.argtypes = [C.c_void_p, C.POINTER(_ChannelLevels), C.c_uint32]
     L.vdl2gpu_get_tables.argtypes = [C.c_void_p] + [C.c_void_p] * 8
     L.vdl2gpu_read_dec.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]
     L.vdl2gpu_read_events.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
@@ -207,6 +215,21 @@ def level_metrics(rec):
                 dc_q=int(rec["sum_q"]) / (n * fs), clipped_fraction=int(rec["clipped"]) / n, peak=int(rec["peak"]) / fs)
 
 
+def channel_level_metrics(rec):
+    """What an operator reads off one record of channel_levels(): samples (the sum of hist), mean in-band power in dBFS
+    (10 log10 of pow / 2^48 / samples; -inf for digital silence), peak in dBFS (10 log10 of peak_pow), noise floor in dBFS
+    (nf_pwr_dbfs) and bin_floor_dbfs, the lower edge of each histogram bin in dBFS (bin 0 has none: -inf).  Power and peak
+    are None for a channel that has measured nothing yet."""
+    n = int(np.asarray(rec["hist"], np.uint64).astype(object).sum())
+    edges = np.concatenate([[-np.inf], 10.0 * np.log10(2.0) * np.arange(-36, 3, dtype=np.float64)])
+    if n == 0:
+        return dict(samples=0, power_dbfs=None, peak_dbfs=None, nf_dbfs=float(rec["nf_pwr_dbfs"]), bin_floor_dbfs=edges)
+    pw = int(rec["pow"]) / float(1 << 48) / n
+    pk = float(rec["peak_pow"])
+    return dict(samples=n, power_dbfs=10.0 * np.log10(pw) if pw > 0 else float("-inf"),
+                peak_dbfs=10.0 * np.log10(pk) if pk > 0 else float("-inf"), nf_dbfs=float(rec["nf_pwr_dbfs"]), bin_floor_dbfs=edges)
+
+
 def make_config(sample_rate, oversample, sample_fmt, centerfreq, freqs, max_ppm=0.0, flags=0):
     """(vdl2gpu_config, the freqs array it points at) for the stage stubs"""
     fr = np.ascontiguousarray(freqs, dtype=np.uint32)
@@ -232,11 +255,14 @@ class Vdl2Channels:
     """N VDL2 channels demodulated from one IQ stream on one H100."""
 
     def __init__(self, sample_rate, oversample, sample_fmt, centerfreq, freqs, max_ppm=0.0,
-                 max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, n_streams=1, levels=False):
+                 max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, n_streams=1, levels=False, channel_levels=False):
         """n_streams > 1: independent-streams mode, channels [s*C, (s+1)*C) demodulate stream s; process_buf_* then take
-        the S per-stream buffers back to back.  levels=True: measure every input's levels (input_levels())."""
+        the S per-stream buffers back to back.  levels=True: measure every input's levels (input_levels());
+        channel_levels=True: measure every channel's in-band levels (channel_levels())."""
         if levels:
             flags |= FLAG_INPUT_LEVELS
+        if channel_levels:
+            flags |= FLAG_CHANNEL_LEVELS
         self.L = load_library()
         self.n_streams = int(n_streams)
         self.freqs = np.ascontiguousarray(freqs, dtype=np.uint32)
@@ -384,6 +410,17 @@ class Vdl2Channels:
         return [dict(samples=o.samples, sum_i=o.sum_i, sum_q=o.sum_q, pow=(o.pow_hi << 64) | o.pow_lo, clipped=o.clipped,
                      peak=o.peak, full_scale=o.full_scale) for o in out[:n]]
 
+    def channel_levels(self):
+        """one dict per channel of what the device measured over every decimated sample submitted so far: hist (uint64
+        array of 40 bins by octave of the sample power p), pow (the 128-bit sum of p x 2^48, truncated per sample, as a
+        Python int), peak_pow, mag_lp, mag_nf and nf_pwr_dbfs (see vdl2gpu_get_channel_levels; channel_level_metrics()
+        turns one into dBFS).  Needs channel_levels=True at creation."""
+        n = self.n_channels
+        out = (_ChannelLevels * max(n, 1))()
+        _check(self.L, self.L.vdl2gpu_get_channel_levels(self.h, out, n), "vdl2gpu_get_channel_levels")
+        return [dict(hist=np.array(o.hist[:], np.uint64), pow=(o.pow_hi << 64) | o.pow_lo, peak_pow=np.float32(o.peak_pow),
+                     mag_lp=np.float32(o.mag_lp), mag_nf=np.float32(o.mag_nf), nf_pwr_dbfs=np.float32(o.nf_pwr_dbfs)) for o in out[:n]]
+
     def kernel_ms(self):
         ms = (C.c_double * 5)()
         n = (C.c_uint64 * 5)()
@@ -397,10 +434,13 @@ class Vdl2Receivers(Vdl2Channels):
     channels_of(r).  The receivers advance in lock step: submit() takes one equal-length buffer per receiver."""
 
     def __init__(self, sample_rate, oversample, sample_fmt, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1,
-                 flags=0, n_inflight=4, levels=False):
-        """receivers: list of (centerfreq, [channel freqs...]); levels=True: measure every receiver's input levels"""
+                 flags=0, n_inflight=4, levels=False, channel_levels=False):
+        """receivers: list of (centerfreq, [channel freqs...]); levels=True: measure every receiver's input levels;
+        channel_levels=True: every channel's in-band levels"""
         if levels:
             flags |= FLAG_INPUT_LEVELS
+        if channel_levels:
+            flags |= FLAG_CHANNEL_LEVELS
         self.L = load_library()
         self.receivers = [(int(cf), [int(f) for f in fr]) for cf, fr in receivers]
         self.n_receivers = self.n_streams = len(self.receivers)
@@ -463,13 +503,16 @@ class Vdl2MixedReceivers(Vdl2Receivers):
     remove_receivers() let receivers join and leave (after flush()) while the others carry on."""
 
     def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, ragged=False,
-                 levels=False):
+                 levels=False, channel_levels=False):
         """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16));
-        levels=True: measure every receiver's input levels (input_levels())"""
+        levels=True: measure every receiver's input levels (input_levels()); channel_levels=True: every channel's in-band
+        levels (channel_levels())"""
         if ragged:
             flags |= FLAG_RAGGED
         if levels:
             flags |= FLAG_INPUT_LEVELS
+        if channel_levels:
+            flags |= FLAG_CHANNEL_LEVELS
         self.ragged = bool(flags & FLAG_RAGGED)
         self.L = load_library()
         rxs = self._normalise(receivers)

@@ -1555,4 +1555,40 @@ VDL2_HD void vdl2_pow_fold(uint64_t &lo, uint64_t &hi, uint64_t v) {
 	hi += vdl2_pow_carry(old, v);
 }
 
+/* ------------------------------------------------------------------------------------------------
+ * Channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS): every decimated sample's power p = fl32(fl32(re re) + fl32(im im)), no FMA,
+ * the reference's symbol power (src/demod.c:266), on the dBFS scale of frame_pwr.  The levels form of K2a adds, per slot,
+ * a histogram of p by octave, the 128-bit sum of q = (uint64)(p 2^48) and the largest p (as float bits: p >= 0, so the
+ * bits order like the values) to planes of uint64 [VDL2_CHLV_ROWS][n_chp] followed by uint32 [n_chp] (the peak).
+ * ---------------------------------------------------------------------------------------------- */
+#define VDL2_CHLV_BINS 40
+#define VDL2_CHLV_POW_LO VDL2_CHLV_BINS         /* rows of the uint64 plane: bins, then the power's low and high words */
+#define VDL2_CHLV_POW_HI (VDL2_CHLV_BINS + 1)
+#define VDL2_CHLV_ROWS (VDL2_CHLV_BINS + 2)
+
+VDL2_HD uint32_t vdl2_f32_bits(float f) {
+#if defined(__CUDA_ARCH__)
+	return __float_as_uint(f);
+#else
+	uint32_t u;
+	memcpy(&u, &f, 4);
+	return u;
+#endif
+}
+VDL2_HD float vdl2_chlv_pow(float re, float im) { return F_ADD(F_MUL(re, re), F_MUL(im, im)); }
+/* from the biased exponent E alone: [0] p < 2^-36 (zeros and subnormals included), [b] 2^(b-37) <= p < 2^(b-36) for
+ * b = 1..38, [39] p >= 2^2 */
+VDL2_HD uint32_t vdl2_chlv_bin(float p) {
+	const int32_t e = (int32_t)((vdl2_f32_bits(p) >> 23) & 0xFFu) - 90;
+	return (uint32_t)(e < 0 ? 0 : e > VDL2_CHLV_BINS - 1 ? VDL2_CHLV_BINS - 1 : e);
+}
+/* p 2^48 truncated: the scaling is exact, and p < 2^15 for every decimated sample (inputs within full scale), so q < 2^63 */
+VDL2_HD uint64_t vdl2_chlv_q(float p) {
+#if defined(__CUDA_ARCH__)
+	return __float2ull_rz(p * 281474976710656.0f);
+#else
+	return (uint64_t)(p * 281474976710656.0f);
+#endif
+}
+
 #endif

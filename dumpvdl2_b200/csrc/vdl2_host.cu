@@ -189,12 +189,17 @@ struct vdl2gpu_ctx {
 	/* input levels (VDL2GPU_FLAG_INPUT_LEVELS; NULL otherwise): one accumulator per input (stream or receiver), which the
 	 * levels form of K0 adds every converted sample to */
 	vdl2_levels *d_levels = nullptr;
+	/* channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS; NULL otherwise): the per-slot planes the levels form of K2a adds every
+	 * decimated sample to, uint64 [VDL2_CHLV_ROWS][n_chp] then the uint32 peak plane [n_chp] */
+	uint64_t *d_chlv = nullptr;
 };
 
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
 		uint32_t n_chp, uint32_t lanes, uint32_t full_warps, std::vector<uint32_t> &k1, std::vector<uint32_t> &k2);
 /* channel -> slot: the first full_warps warps hold `lanes` channels each, the others lanes - 1 */
 static inline uint32_t slot_of(uint32_t ch, uint32_t lanes, uint32_t full_warps) { return vdl2_channel_slot(ch, lanes, full_warps); }
+/* the noise floor in dBFS, of a frame and of vdl2gpu_get_channel_levels (src/decode.c:181) */
+static inline float nf_pwr_dbfs(float mag_nf) { return 20.0f * log10f(mag_nf + 0.001f); }
 
 extern "C" int vdl2gpu_abi_version(void) { return VDL2GPU_ABI_VERSION; }
 
@@ -248,7 +253,7 @@ static void free_layout(vdl2gpu_ctx *c) {
 	cudaFree(c->d_counters); cudaFree(c->d_ready); cudaFree(c->d_ring); cudaFree(c->d_pool); cudaFree(c->d_free); cudaFree(c->d_ctl);
 	cudaFree(c->d_slot_rx); cudaFree(c->d_block_rx);
 	cudaFree(c->d_rx_in); cudaFree(c->d_slot_cls);
-	cudaFree(c->d_levels);
+	cudaFree(c->d_levels); cudaFree(c->d_chlv);
 }
 
 /* the pushed-input rings and their queues (no push, copy or span may be running on them) */
@@ -427,6 +432,11 @@ static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu
 		CU(cudaMalloc(&c->d_levels, (size_t)c->n_streams * sizeof(vdl2_levels)));
 		CU(cudaMemset(c->d_levels, 0, (size_t)c->n_streams * sizeof(vdl2_levels)));
 	}
+	if(c->cfg.flags & VDL2GPU_FLAG_CHANNEL_LEVELS) {
+		const size_t bytes = (size_t)VDL2_CHLV_ROWS * c->n_chp * 8 + (size_t)c->n_chp * 4;
+		CU(cudaMalloc(&c->d_chlv, bytes));
+		CU(cudaMemset(c->d_chlv, 0, bytes));
+	}
 	if(c->mixed) {
 		CU(cudaMalloc(&c->d_rx_in, c->rx_in.size() * sizeof(vdl2_rx_input)));
 		CU(cudaMalloc(&c->d_slot_cls, slot_cls.size()));
@@ -476,7 +486,7 @@ static void swap_layout(vdl2gpu_ctx *a, vdl2gpu_ctx *b) {
 	swap(a->d_samples, b->d_samples); swap(a->d_dec3, b->d_dec3); swap(a->d_phase2, b->d_phase2); swap(a->d_mag2, b->d_mag2);
 	swap(a->d_k1, b->d_k1); swap(a->d_k2, b->d_k2); swap(a->d_counters, b->d_counters); swap(a->d_ring, b->d_ring);
 	swap(a->d_pool, b->d_pool); swap(a->d_free, b->d_free); swap(a->d_ready, b->d_ready); swap(a->d_ctl, b->d_ctl);
-	swap(a->d_levels, b->d_levels);
+	swap(a->d_levels, b->d_levels); swap(a->d_chlv, b->d_chlv);
 	swap(a->chunks, b->chunks);
 }
 
@@ -755,7 +765,7 @@ static void parse_region(const uint8_t *region, uint32_t out_cap, double rate, s
 			pf.f.num_fec_corrections = r->num_fec_corrections;
 			pf.f.frame_pwr = r->frame_pwr; pf.f.mag_nf = r->mag_nf;
 			pf.f.frame_pwr_dbfs = 10.0f * log10f(r->frame_pwr);                  /* src/decode.c:180 */
-			pf.f.nf_pwr_dbfs = 20.0f * log10f(r->mag_nf + 0.001f);               /* src/decode.c:181 */
+			pf.f.nf_pwr_dbfs = nf_pwr_dbfs(r->mag_nf);
 			pf.f.ppm_error = r->ppm_error;
 			pf.f.sync_dec_index = sync_idx;
 			/* the reference stamps gettimeofday() at sync (src/demod.c:246); here: arrival time of the chunk
@@ -899,7 +909,7 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	const bool need_mag = (c->k2_variant & 0xFF) >= 0 && (c->k2_variant & 0xFF) <= 4;
 	pa.dec = d_dec; pa.phase = c->d_phase2[pb]; pa.mag = need_mag ? c->d_mag2[pb] : nullptr; pa.phase_prev = c->d_phase2[pb ^ 1];
 	pa.n_dec = n_dec; pa.prev_n_dec = prev_n_dec; pa.n_ch = c->n_ch; pa.n_chp = c->n_chp; pa.lanes = c->lanes; pa.full_warps = c->full_warps;
-	pa.mode = (uint32_t)c->k2a_mode; pa.split = c->k2a_split; pa.ca = ca;
+	pa.mode = (uint32_t)c->k2a_mode; pa.split = c->k2a_split; pa.ca = ca; pa.chlv = c->d_chlv;
 	p2.dec = d_dec; p2.phase = c->d_phase2[pb]; p2.mag = c->d_mag2[pb]; p2.hist_tmp = nullptr; p2.n_dec = n_dec; p2.n_ch = c->n_ch; p2.n_chp = c->n_chp;
 	p2.lanes = c->lanes; p2.full_warps = c->full_warps; p2.dec_base = dec_base;
 	p2.state = c->d_k2; p2.ring = c->d_ring; p2.tables = c->d_tab; p2.max_ppm = c->cfg.max_ppm; p2.s27 = c->tab.s27;
@@ -1602,6 +1612,7 @@ static int migrate_receivers(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const vdl2gpu_recei
 	p.n_chp = n->n_chp; p.old_n_chp = c->n_chp;
 	p.old_k1 = c->d_k1; p.old_k2 = c->d_k2; p.old_counters = c->d_counters; p.old_ring = c->d_ring; p.old_phase = c->d_phase2[pb_prev];
 	p.k1 = n->d_k1; p.k2 = n->d_k2; p.counters = n->d_counters; p.ring = n->d_ring; p.phase = n->d_phase2[pb_prev];
+	p.old_chlv = c->d_chlv; p.chlv = n->d_chlv;                  /* (channel levels: both NULL or both allocated) */
 	KL(vdl2_launch_migrate(&p, c->stream));
 	/* held slots keep their indices (and their words): K2 writes a burst's channel number into its slot only at hand-off */
 	CU(cudaMemcpyAsync(n->d_pool, c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot), cudaMemcpyDeviceToDevice, c->stream));
@@ -1856,6 +1867,40 @@ extern "C" int vdl2gpu_get_input_levels(vdl2gpu_ctx *c, vdl2gpu_input_levels *ou
 		o.clipped = lv[k].clipped;
 		o.peak = lv[k].peak;
 		o.full_scale = vdl2_level_full_scale(c->mixed ? c->rx_in[k].fmt : c->cfg.sample_fmt);
+	}
+	return VDL2GPU_OK;
+}
+
+/* Channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS): out[k] for the first n channels, after everything submitted so far has run */
+extern "C" int vdl2gpu_get_channel_levels(vdl2gpu_ctx *c, vdl2gpu_channel_levels *out, uint32_t n) {
+	const char *why = nullptr;
+	if(!c) why = "no context";
+	else if(!out) why = "no output";
+	else if(!c->d_chlv) why = "the context was created without VDL2GPU_FLAG_CHANNEL_LEVELS";
+	else if(n > c->n_ch) why = "more channels asked for than the context has";
+	if(why) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_get_channel_levels: %s", why);
+		return VDL2GPU_EINVAL;
+	}
+	if(n == 0) return VDL2GPU_OK;
+	CU(cudaSetDevice(c->device));
+	CU(cudaStreamSynchronize(c->stream));
+	CU(cudaStreamSynchronize(c->s_back));
+	const size_t s = c->n_chp;
+	std::vector<uint64_t> lv(VDL2_CHLV_ROWS * s);
+	std::vector<uint32_t> peak(s), nf(2 * s);
+	CU(cudaMemcpy(lv.data(), c->d_chlv, lv.size() * 8, cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy(peak.data(), c->d_chlv + VDL2_CHLV_ROWS * s, s * 4, cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy(nf.data(), c->d_k2 + (size_t)K2_MAG_LP * s, 2 * s * 4, cudaMemcpyDeviceToHost));     /* K2_MAG_LP, K2_MAG_NF */
+	for(uint32_t k = 0; k < n; k++) {
+		const size_t i = slot_of(k, c->lanes, c->full_warps);
+		vdl2gpu_channel_levels &o = out[k];
+		for(int b = 0; b < VDL2_CHLV_BINS; b++) o.hist[b] = lv[b * s + i];
+		o.pow_lo = lv[VDL2_CHLV_POW_LO * s + i]; o.pow_hi = lv[VDL2_CHLV_POW_HI * s + i];
+		memcpy(&o.peak_pow, &peak[i], 4);
+		memcpy(&o.mag_lp, &nf[i], 4);
+		memcpy(&o.mag_nf, &nf[s + i], 4);
+		o.nf_pwr_dbfs = nf_pwr_dbfs(o.mag_nf);
 	}
 	return VDL2GPU_OK;
 }

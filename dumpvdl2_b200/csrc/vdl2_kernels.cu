@@ -1096,9 +1096,15 @@ __global__ void __launch_bounds__(256) k2a_phase_mag(const float2 *__restrict__ 
  * span) the range is the previous plane's own history rows, which are the right ones; with 0 < prev_n < 160 it straddles
  * history and new rows, still in order.  So the two alternating planes need no change for ragged spans.  A lane whose
  * channel restarts with the span (p.rx_restart) writes zero history rows instead: the new process has no past. */
-template<bool FAST, bool RAGGED>
+/* Channel levels (LEVELS, VDL2GPU_FLAG_CHANNEL_LEVELS): every sample a thread evaluates also goes into its slice's figures.
+ * The histogram sits in shared memory, one column per thread (bank = lane, no atomics); the 128-bit power sum (folded
+ * per sample: q < 2^63, so two loud samples can wrap 64 bits) and the peak sit in registers.  At the end of its slice the
+ * thread adds its non-zero bins, its power and its peak to its slot's planes with integer atomics (the power's carry as
+ * in vdl2_pow_carry), so the totals are exact in any order of slices and chunks. */
+template<bool FAST, bool RAGGED, bool LEVELS>
 __device__ __forceinline__ void k2a_warps_body(const vdl2_k2a_params &p) {
 	__shared__ double s_atan[VDL2_ATAN_TABLE_DOUBLES];
+	__shared__ uint32_t s_hist[LEVELS ? VDL2_CHLV_BINS : 1][128];
 	if(FAST) {
 		if(threadIdx.x < VDL2_ATAN_TABLE_DOUBLES) s_atan[threadIdx.x] = c_atan_tab[threadIdx.x];
 		__syncthreads();
@@ -1107,6 +1113,18 @@ __device__ __forceinline__ void k2a_warps_body(const vdl2_k2a_params &p) {
 	const uint32_t slot = (blockIdx.x % nblk) * 128u + threadIdx.x;
 	uint32_t chan;
 	if(!vdl2_slot_channel(slot, p.lanes, p.full_warps, p.n_ch, chan)) return;
+	uint64_t lv_lo = 0, lv_hi = 0;
+	uint32_t lv_peak = 0;
+	if(LEVELS) {
+#pragma unroll
+		for(int b = 0; b < VDL2_CHLV_BINS; b++) s_hist[b][threadIdx.x] = 0u;
+	}
+	auto level = [&](float2 d) {
+		const float pw = vdl2_chlv_pow(d.x, d.y);
+		s_hist[vdl2_chlv_bin(pw)][threadIdx.x]++;
+		vdl2_pow_fold(lv_lo, lv_hi, vdl2_chlv_q(pw));
+		lv_peak = max(lv_peak, vdl2_f32_bits(pw));
+	};
 	const uint32_t n_all = p.ca ? p.ca->n_dec : p.n_dec, prev_n_dec = RAGGED ? p.rx_span[p.slot_rx[slot]].prev_n : p.ca ? p.ca->prev_n_dec : p.prev_n_dec;
 	const uint32_t n_mine = RAGGED ? p.rx_span[p.slot_rx[slot]].n : n_all;     /* ragged: n_all is the span's width */
 	/* this block's time slice [t, n_dec) of the chunk, boundaries on multiples of 4 samples (ragged: the width's slices,
@@ -1163,21 +1181,41 @@ __device__ __forceinline__ void k2a_warps_body(const vdl2_k2a_params &p) {
 				if(sm[k]) m[k] = vdl2_mag_of(d[k].x, d[k].y);
 				mg[(size_t)(t + k) * s] = m[k];
 			}
+			if(LEVELS) level(d[k]);
 		}
 	}
 	for(; t < n_dec; t++) {
 		const float2 d = dec[(size_t)t * s];
 		ph[(size_t)t * s] = vdl2_phase_of(d.x, d.y);
 		if(p.mag != nullptr) mg[(size_t)t * s] = vdl2_mag_of(d.x, d.y);
+		if(LEVELS) level(d);
+	}
+	if(LEVELS) {
+		uint64_t *lv = p.chlv + slot;
+#pragma unroll 4
+		for(int b = 0; b < VDL2_CHLV_BINS; b++) {
+			const uint32_t n = s_hist[b][threadIdx.x];
+			if(n) atomicAdd((unsigned long long *)(lv + b * s), (unsigned long long)n);
+		}
+		if(lv_lo != 0u) lv_hi += vdl2_pow_carry(atomicAdd((unsigned long long *)(lv + VDL2_CHLV_POW_LO * s), (unsigned long long)lv_lo), lv_lo);
+		if(lv_hi != 0u) atomicAdd((unsigned long long *)(lv + VDL2_CHLV_POW_HI * s), (unsigned long long)lv_hi);
+		if(lv_peak != 0u) atomicMax(reinterpret_cast<uint32_t *>(p.chlv + VDL2_CHLV_ROWS * s) + slot, lv_peak);
 	}
 }
 
-template<bool FAST>
-__global__ void __launch_bounds__(128, 8) k2a_phase_mag_warps(vdl2_k2a_params p) { k2a_warps_body<FAST, false>(p); }     /* <= 64 registers: 32 warps per SM */
+template<bool FAST, bool LEVELS>
+__global__ void __launch_bounds__(128, LEVELS ? 6 : 8) k2a_phase_mag_warps(vdl2_k2a_params p) { k2a_warps_body<FAST, false, LEVELS>(p); }     /* <= 64 registers: 32 warps per SM */
 /* (the lane's own row count and slice end take two more registers than the uniform ones of the lock-step kernel: within 64
  * the fast form spilled, so seven blocks per SM, <= 72 registers) */
-template<bool FAST>
-__global__ void __launch_bounds__(128, 7) k2a_phase_mag_warps_ragged(vdl2_k2a_params p) { k2a_warps_body<FAST, true>(p); }
+template<bool FAST, bool LEVELS>
+__global__ void __launch_bounds__(128, LEVELS ? 6 : 7) k2a_phase_mag_warps_ragged(vdl2_k2a_params p) { k2a_warps_body<FAST, true, LEVELS>(p); }
+/* (LEVELS: the register partials and the slice's 20 KB histogram; six blocks per SM, <= 80 registers, no spills.  They are
+ * instantiated here, ahead of the launchers: that places their code after every other kernel's in the module, so adding
+ * them left the other kernels' code where it was) */
+template __global__ void k2a_phase_mag_warps<false, true>(vdl2_k2a_params);
+template __global__ void k2a_phase_mag_warps<true, true>(vdl2_k2a_params);
+template __global__ void k2a_phase_mag_warps_ragged<false, true>(vdl2_k2a_params);
+template __global__ void k2a_phase_mag_warps_ragged<true, true>(vdl2_k2a_params);
 
 /* carry the last 160 phase rows over to the front of the plane for the next chunk: rows [n_dec, n_dec+160) -> [0, 160) */
 __global__ void __launch_bounds__(256) k_copy_rows(const float *__restrict__ src, float *__restrict__ dst, uint32_t n) {
@@ -1681,13 +1719,17 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		vdl2_set_carveout(k1_mix_iir_decimate_ragged<false>, pct);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_ragged<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
 		cudaFuncSetAttribute(k1_mix_iir_decimate_ragged<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VDL2_RX_MIXED_SMEM_MAX);
-		vdl2_set_carveout(k2a_phase_mag_warps_ragged<true>, pct);
-		vdl2_set_carveout(k2a_phase_mag_warps_ragged<false>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps_ragged<true, false>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps_ragged<false, false>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps_ragged<true, true>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps_ragged<false, true>, pct);
 		vdl2_set_carveout(k2_sync_slice_ragged, pct);
 		cudaFuncSetAttribute(k2_sync_slice_ragged, cudaFuncAttributeMaxDynamicSharedMemorySize, K2_SMEM_BYTES(K2_BLOCK, 4));
 		vdl2_set_carveout(k2a_phase_mag<true>, pct);
-		vdl2_set_carveout(k2a_phase_mag_warps<true>, pct);
-		vdl2_set_carveout(k2a_phase_mag_warps<false>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps<true, false>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps<false, false>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps<true, true>, pct);
+		vdl2_set_carveout(k2a_phase_mag_warps<false, true>, pct);
 		vdl2_set_carveout(k2a_phase_mag<false>, pct);
 #define K2_SETUP(BLK, BLOCKED, MODE) do { vdl2_set_carveout(k2_sync_slice<BLK, BLOCKED, MODE>, pct); \
 		cudaFuncSetAttribute(k2_sync_slice<BLK, BLOCKED, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, K2_SMEM_BYTES(BLK, MODE)); } while(0)
@@ -1833,11 +1875,12 @@ extern "C" int vdl2_launch_k2a(const vdl2_k2_params *p, cudaStream_t st) {
 extern "C" int vdl2_launch_k2a_warps(const vdl2_k2a_params *p, cudaStream_t st) {
 	if(p->n_ch == 0) return 0;
 	const uint32_t blocks = ((p->n_chp + 127u) / 128u) * (p->split ? p->split : 1u);
-	if(p->rx_span) {                                  /* ragged spans */
-		if(p->mode) k2a_phase_mag_warps_ragged<true><<<blocks, 128, 0, st>>>(*p);
-		else k2a_phase_mag_warps_ragged<false><<<blocks, 128, 0, st>>>(*p);
-	} else if(p->mode) k2a_phase_mag_warps<true><<<blocks, 128, 0, st>>>(*p);
-	else k2a_phase_mag_warps<false><<<blocks, 128, 0, st>>>(*p);
+	const bool lv = p->chlv != nullptr;
+	auto k = p->rx_span ? (p->mode ? (lv ? k2a_phase_mag_warps_ragged<true, true> : k2a_phase_mag_warps_ragged<true, false>)     /* ragged spans */
+			: (lv ? k2a_phase_mag_warps_ragged<false, true> : k2a_phase_mag_warps_ragged<false, false>))
+		: p->mode ? (lv ? k2a_phase_mag_warps<true, true> : k2a_phase_mag_warps<true, false>)
+		: (lv ? k2a_phase_mag_warps<false, true> : k2a_phase_mag_warps<false, false>);
+	k<<<blocks, 128, 0, st>>>(*p);
 	return (int)cudaGetLastError();
 }
 
@@ -1910,6 +1953,7 @@ extern "C" int vdl2_launch_rs(uint8_t *blocks, const int32_t *fec_octets, uint32
  * span would have taken its history from become rows [0, 160) of the new one, which the host then pairs with prev_n = 0.
  * Thread i also fills channel i of the per-channel counters, which are kept by channel.
  * ---------------------------------------------------------------------------------------------- */
+template<bool LEVELS>
 __global__ void __launch_bounds__(256) k_migrate_receivers(vdl2_migrate_params p) {
 	const uint32_t i = blockIdx.x * 256u + threadIdx.x;
 	if(i >= p.n_chp) return;
@@ -1935,9 +1979,15 @@ __global__ void __launch_bounds__(256) k_migrate_receivers(vdl2_migrate_params p
 		for(uint32_t t = 0; t < VDL2_SYNC_BUFLEN; t++) { p.ring[t * s + i] = 0.f; p.phase[t * s + i] = 0.f; }
 	}
 	for(int k = 0; k < VDL2_NUM_COUNTERS; k++) p.counters[k * s + i] = m.chan_from >= 0 ? p.old_counters[k * so + (size_t)m.chan_from] : 0u;
+	if(LEVELS) {                                  /* channel levels, by slot: a kept slot carries them, any other starts at zero */
+		for(int r = 0; r < VDL2_CHLV_ROWS; r++) p.chlv[r * s + i] = m.slot_from >= 0 ? p.old_chlv[r * so + m.slot_from] : 0u;
+		reinterpret_cast<uint32_t *>(p.chlv + VDL2_CHLV_ROWS * s)[i] =
+				m.slot_from >= 0 ? reinterpret_cast<const uint32_t *>(p.old_chlv + VDL2_CHLV_ROWS * so)[m.slot_from] : 0u;
+	}
 }
 
 extern "C" int vdl2_launch_migrate(const vdl2_migrate_params *p, cudaStream_t st) {
-	k_migrate_receivers<<<(p->n_chp + 255u) / 256u, 256, 0, st>>>(*p);
+	if(p->chlv) k_migrate_receivers<true><<<(p->n_chp + 255u) / 256u, 256, 0, st>>>(*p);
+	else k_migrate_receivers<false><<<(p->n_chp + 255u) / 256u, 256, 0, st>>>(*p);
 	return (int)cudaGetLastError();
 }

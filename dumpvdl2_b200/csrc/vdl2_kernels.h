@@ -122,6 +122,9 @@ typedef struct {
 	const vdl2_rx_span *rx_span;
 	/* (NULL unless the span restarts receivers) per slot: zero history rows instead of the previous plane's */
 	const vdl2_rx_restart *rx_restart;
+	/* channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS; NULL otherwise): uint64 [VDL2_CHLV_ROWS][n_chp] then the uint32 peak plane
+	 * [n_chp], which the levels form adds every sample it evaluates to (vdl2_core.cuh) */
+	uint64_t *chlv;
 } vdl2_k2a_params;
 
 typedef struct {
@@ -147,6 +150,8 @@ typedef struct {
 	const float *old_phase;      /* the old plane the next span would have taken its history rows from */
 	uint32_t *k1, *k2, *counters;
 	float *ring, *phase;         /* phase: the new plane the next span takes its history rows from */
+	const uint64_t *old_chlv;    /* channel levels planes by slot (vdl2_k2a_params.chlv), or NULL */
+	uint64_t *chlv;
 } vdl2_migrate_params;
 
 #ifdef __cplusplus

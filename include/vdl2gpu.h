@@ -54,7 +54,9 @@ enum {
 	VDL2GPU_FLAG_NO_GRAPH = 1u << 4,     /* launch every kernel individually instead of replaying the per-chunk CUDA graphs */
 	VDL2GPU_FLAG_RAGGED = 1u << 5,       /* vdl2gpu_create_mixed_receivers only: every receiver brings its own number of decimated
 	                                      * samples to a span (vdl2gpu_submit_ragged); every other create function refuses it */
-	VDL2GPU_FLAG_INPUT_LEVELS = 1u << 6  /* measure every input's levels on the device (vdl2gpu_get_input_levels); any create function */
+	VDL2GPU_FLAG_INPUT_LEVELS = 1u << 6, /* measure every input's levels on the device (vdl2gpu_get_input_levels); any create function */
+	VDL2GPU_FLAG_CHANNEL_LEVELS = 1u << 7 /* measure every channel's in-band levels on the device (vdl2gpu_get_channel_levels); any
+	                                       * create function */
 };
 
 typedef struct {
@@ -356,6 +358,37 @@ typedef struct {
  * vdl2gpu_last_error) for a NULL context or output, n larger than the number of inputs, or a context created without
  * VDL2GPU_FLAG_INPUT_LEVELS.  Not available through the stage stubs or the drop-in symbols. */
 int vdl2gpu_get_input_levels(vdl2gpu_ctx *ctx, vdl2gpu_input_levels *out, uint32_t n);
+
+/* Channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS): what every channel hears in its band, for telling a raised noise floor or a
+ * parked carrier from a quiet sky on a channel that sends no frames.  p = fl32(fl32(re x re) + fl32(im x im)), without FMA,
+ * of a decimated sample is the reference's symbol power (src/demod.c:266): 10 log10(p) is on the dBFS scale of a frame's
+ * frame_pwr_dbfs.  Its bin comes from the biased exponent E of p alone, b = min(max(E - 90, 0), 39): bins 3.01 dB wide
+ * covering -108.4 to +6.0 dBFS.  q = (uint64)(p x 2^48), truncated; p < 2^15 for every decimated sample, so q fits. */
+typedef struct {
+	uint64_t hist[40];           /* decimated samples by octave of p: [0] p < 2^-36 (zeros included),
+	                              * [b] 2^(b-37) <= p < 2^(b-36) for b = 1..38, [39] p >= 2^2; their sum is the sample count */
+	uint64_t pow_lo, pow_hi;     /* sum over those samples of q, one unsigned 128-bit integer */
+	float peak_pow;              /* largest p */
+	float mag_lp, mag_nf;        /* the channel's noise-floor filters as they stand now (src/demod.c:238-243) */
+	float nf_pwr_dbfs;           /* 20 log10f(mag_nf + 0.001f), computed as for a frame's nf_pwr_dbfs */
+} vdl2gpu_channel_levels;        /* 352 bytes */
+/* out[k] = the levels of channel k (its index into cfg->freqs) for k < n.
+ *   - Cumulative from create (for a channel added by vdl2gpu_update_receivers: from when it joined), over every decimated
+ *     sample of every chunk or span submitted before the call; the call waits for that work.  Take windows by
+ *     differencing two reads.
+ *   - The integers and peak_pow are exact and do not depend on chunk, span or push lengths, ragged counts, n_inflight,
+ *     graphs, trace or how the phase pass is cut in time (VDL2GPU_K2A_SPLIT, VDL2GPU_STAGES=3).  Ragged spans count only
+ *     the rows a receiver brought.
+ *   - vdl2gpu_restart_receiver: hist, power and peak keep counting, as the per-channel counters do; mag_lp and mag_nf are
+ *     the new process's, which starts at 0 and 2.0 as the reference's does (src/demod.c:383).
+ *   - vdl2gpu_update_receivers: a kept channel carries its levels to its new index, a new channel starts at zero, a
+ *     removed channel's levels are gone.
+ *   - Frames, metadata, counters, trace events and vdl2gpu_stats are the same with the flag on or off.  A context without
+ *     the flag allocates and launches nothing for it.
+ * Runs on the control thread, concurrently with vdl2gpu_push.  VDL2GPU_EINVAL (with vdl2gpu_last_error) for a NULL context
+ * or output, n larger than the number of channels, or a context created without VDL2GPU_FLAG_CHANNEL_LEVELS.  Not
+ * available through the stage stubs or the drop-in symbols. */
+int vdl2gpu_get_channel_levels(vdl2gpu_ctx *ctx, vdl2gpu_channel_levels *out, uint32_t n);
 
 /* ---- multi-GPU ingest (one process per GPU; global channel k is demodulated on GPU k mod N, the reference's
  * channel threads share nothing but the read-only sample buffer: src/dumpvdl2.c:117-135, src/demod.c:50,300-301).
