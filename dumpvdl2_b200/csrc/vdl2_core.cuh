@@ -463,9 +463,9 @@ VDL2_HD void vdl2_init_eval(vdl2_chan &v, const float *ring, int rs, const vdl2_
 	}
 }
 
-/* DM_SYNC, every SPS-th sample: one D8PSK symbol, src/demod.c:256-283 */
-VDL2_HD void vdl2_symbol(vdl2_chan &v, const vdl2_k2_env &env, uint32_t chan_idx, uint64_t dec_index,
-		float re, float im, float phi) {
+/* DM_SYNC, every SPS-th sample: one D8PSK symbol, src/demod.c:256-283: slicing, frame power and bit packing (vdl2_symbol
+ * without what a full bit count triggers) */
+VDL2_HD void vdl2_symbol_bits(vdl2_chan &v, const vdl2_k2_env &env, float re, float im, float phi) {
 	float dphi = F_SUB(F_SUB(phi, v.prev_phi), v.dphi);
 	if(dphi < 0.f) dphi = D_TO_F(D_ADD((double)dphi, VDL2_TWO_PI));
 	else if(dphi >= VDL2_TWO_PI_F_ABOVE) dphi = D_TO_F(D_SUB((double)dphi, VDL2_TWO_PI));
@@ -483,6 +483,11 @@ VDL2_HD void vdl2_symbol(vdl2_chan &v, const vdl2_k2_env &env, uint32_t chan_idx
 	v.nbits = before + 3;
 	if((before >> 5) != (v.nbits >> 5) && v.slot >= 0)
 		env.pool[v.slot].words[before >> 5] = (uint32_t)(v.acc >> (v.nbits & 31u));
+}
+
+VDL2_HD void vdl2_symbol(vdl2_chan &v, const vdl2_k2_env &env, uint32_t chan_idx, uint64_t dec_index,
+		float re, float im, float phi) {
+	vdl2_symbol_bits(v, env, re, im, phi);
 	if(v.nbits >= v.need_bits) {
 		if(vdl2_dec_state(v) == VDL2_DEC_HEADER) vdl2_header_step(v, env, chan_idx, dec_index);
 		else if(vdl2_dec_state(v) == VDL2_DEC_DATA) vdl2_burst_complete(v, env, chan_idx);
@@ -770,6 +775,113 @@ VDL2_HD void vdl2_walk_block_ring(vdl2_chan &v, float *ring, int rs, const vdl2_
 		}
 	}
 	vdl2_walk_tail<STAGED>(v, ring, rs, env, chan_idx, idx0, dec, phase, mag, stride, resume);
+}
+
+/* Data symbols sliced after the walk (the default walk, k2_sync_slice<128, true, 4> and k2_sync_slice_ragged).
+ *
+ * Once the header has fixed a burst's length, its data symbols depend on nothing else the walk does: symbol k reads its
+ * own sample and phase and symbol k-1's phase from the planes, `dphi` and the sample clock; only frame_pwr, the bit
+ * accumulator and the pool words chain from one symbol to the next, and while locked no ring slot, mag_lp or nfcnt changes.
+ * With the 32 lanes of a warp on 32 different signals almost every block has a lane inside a burst, and slicing its
+ * symbols there kept the other 31 idle behind a serial FP64 chain per symbol.  So a lane in DEC_DATA skips its blocks
+ * (only the sample clock is implied: the burst's last symbol falls at a known sample), and the symbols are sliced after
+ * the block loop, for all lanes of the warp together, by the same vdl2_symbol operations in the same order:
+ *   - a burst that ends inside the launch, followed by at least one more sample, is queued: its state before the first
+ *     pending symbol is kept (`q`, one burst per lane); the lane takes what the last symbol leaves behind that the next
+ *     sample's demod_reset does not clear (prev_phi, burst_seq, slot, IDLE, sclk) and walks on.  With the queue taken, the
+ *     burst is sliced at once instead.  A burst without a pool slot (slot < 0) writes nothing: it needs no queue.
+ *   - a burst still open at the launch's end (its last symbol on the launch's last sample or later) is sliced up to its
+ *     last symbol in the launch, on the lane's own state.
+ * Every field of the channel, its ring and the pool words are at the end of a launch what the inline walk leaves; only
+ * the order of ready-list entries within a launch differs, and K3 decodes the list in any order. */
+struct vdl2_defer {
+	int32_t at;          /* launch-local sample of the next unsliced symbol of the burst the lane is in; < 0: none */
+	int32_t last;        /* launch-local sample of that burst's last symbol */
+	int32_t q_at;        /* queued burst: sample of its first unsliced symbol; < 0: the queue is empty */
+	vdl2_chan q;         /* the queued burst's state before that symbol */
+};
+
+VDL2_HD void vdl2_defer_init(vdl2_defer &d) { d.at = -1; d.last = -1; d.q_at = -1; }
+
+/* sample of the last symbol of the burst whose next symbol falls at sample `at` */
+VDL2_HD int vdl2_burst_last(const vdl2_chan &v, int at) {
+	return at + VDL2_SPS * ((int)((v.need_bits - v.nbits + 2u) / 3u) - 1);
+}
+
+/* at launch-local sample m, before it is walked: a lane that is in a burst's data part starts skipping */
+VDL2_HD void vdl2_defer_enter(vdl2_defer &d, const vdl2_chan &v, int m) {
+	if(d.at < 0 && (v.state & VDL2_ST_LOCKED) && vdl2_dec_state(v) == VDL2_DEC_DATA) {
+		d.at = m + (VDL2_SPS - 1) - v.sclk;                    /* the sample on which ++sclk reaches SPS */
+		d.last = vdl2_burst_last(v, d.at);
+	}
+}
+
+/* slice the symbols at samples at, at + SPS, ... < end of a channel in DEC_DATA (vdl2_symbol; a data symbol emits no event);
+ * returns the sample of the next one.  dec / phase: the lane's launch-local sample 0, consecutive samples `stride` apart */
+VDL2_HD int vdl2_slice_run(vdl2_chan &w, const vdl2_k2_env &env, uint32_t chan_idx, const float2 *dec, const float *phase,
+		size_t stride, int at, int end) {
+	for(; at < end; at += VDL2_SPS) {
+		const float2 d = VDL2_LDG(dec + (ptrdiff_t)at * (ptrdiff_t)stride);
+		const float phi = VDL2_LDG(phase + (ptrdiff_t)at * (ptrdiff_t)stride);
+		w.sclk = 0;
+		vdl2_symbol_bits(w, env, d.x, d.y, phi);
+		if(w.nbits >= w.need_bits) vdl2_burst_complete(w, env, chan_idx);
+	}
+	return at;
+}
+
+/* the lane's burst ends on sample d.last and the walk goes on at d.last + 1; last_phi = that sample's phase */
+VDL2_HD void vdl2_defer_burst_end(vdl2_defer &d, vdl2_chan &v, const vdl2_k2_env &env, uint32_t chan_idx,
+		const float2 *dec, const float *phase, size_t stride, float last_phi) {
+	if(v.slot >= 0 && d.q_at >= 0) {
+		vdl2_slice_run(v, env, chan_idx, dec, phase, stride, d.at, d.last + 1);      /* queue taken: slice it now */
+	} else {
+		if(v.slot >= 0) { d.q = v; d.q_at = d.at; v.slot = -1; }
+		/* the rest of what the last symbol leaves (vdl2_burst_complete) is cleared by the next sample's demod_reset */
+		v.prev_phi = last_phi;
+		v.sclk = 0;
+		v.burst_seq++;
+		vdl2_set_dec_state(v, VDL2_DEC_IDLE);
+	}
+	d.at = -1;
+}
+
+/* after the walk of a launch of n_dec samples: the queued burst, then the one still open */
+VDL2_HD void vdl2_defer_finish(vdl2_defer &d, vdl2_chan &v, const vdl2_k2_env &env, uint32_t chan_idx,
+		const float2 *dec, const float *phase, size_t stride, int n_dec) {
+	if(d.q_at >= 0) vdl2_slice_run(d.q, env, chan_idx, dec, phase, stride, d.q_at, vdl2_burst_last(d.q, d.q_at) + 1);
+	if(d.at >= 0) {
+		const int next = vdl2_slice_run(v, env, chan_idx, dec, phase, stride, d.at, d.last < n_dec ? d.last + 1 : n_dec);
+		v.sclk = (VDL2_SPS - 1) + n_dec - next;               /* samples since the last symbol, as ++sclk would count them */
+	}
+	vdl2_defer_init(d);
+}
+
+/* the default walk's block at launch-local sample m with the lane deferring: false when the block is not taken here.  The
+ * lane skips the block while its burst goes on past it or to the launch's end; when the burst ends in the block, the rest
+ * of the block is walked per sample.  bdec / bphase: the block's samples, `bs` apart (STAGED: shared memory) */
+template<bool STAGED>
+VDL2_HD bool vdl2_defer_block(vdl2_defer &d, vdl2_chan &v, float *ring, int rs, const vdl2_k2_env &env, uint32_t chan_idx,
+		uint64_t idx0, int m, int n_dec, const float2 *bdec, const float *bphase, size_t bs,
+		const float2 *dec, const float *phase, size_t stride) {
+	vdl2_defer_enter(d, v, m);
+	if(d.at < 0) return false;
+	const int t = d.last - m;
+	if(t >= VDL2_WALK_BLOCK || d.last + 1 >= n_dec) return true;
+	vdl2_defer_burst_end(d, v, env, chan_idx, dec, phase, stride, VDL2_LD(STAGED, bphase + (ptrdiff_t)t * (ptrdiff_t)bs));
+	vdl2_walk_tail<STAGED>(v, ring, rs, env, chan_idx, idx0, bdec, bphase, nullptr, bs, t + 1);
+	return true;
+}
+
+/* the same for one sample of the per-sample tail: returns the next sample to walk (n_dec: the walk is done) or -1 when
+ * sample m is not taken here */
+VDL2_HD int vdl2_defer_sample(vdl2_defer &d, vdl2_chan &v, const vdl2_k2_env &env, uint32_t chan_idx, int m, int n_dec,
+		const float2 *dec, const float *phase, size_t stride) {
+	vdl2_defer_enter(d, v, m);
+	if(d.at < 0) return -1;
+	if(d.last + 1 >= n_dec) return n_dec;
+	vdl2_defer_burst_end(d, v, env, chan_idx, dec, phase, stride, VDL2_LDG(phase + (ptrdiff_t)d.last * (ptrdiff_t)stride));
+	return d.last + 1;
 }
 
 /* same, computing phase and magnitude in place (host simulation, unit tests) */

@@ -1317,6 +1317,11 @@ __device__ __forceinline__ void k2_sync_body(const vdl2_k2_params &p) {
 	const float *mgs = p.mag + ch;
 	const uint32_t n_dec = RAGGED ? p.rx_span[p.slot_rx[ch]].n : p.ca ? p.ca->n_dec : p.n_dec;
 	const uint64_t dec_base = RAGGED ? p.rx_span[p.slot_rx[ch]].dec_base : p.ca ? p.ca->dec_base : p.dec_base;
+	/* DEFER: a lane inside a burst's data part skips its blocks, the symbols are sliced after the walk (vdl2_defer, vdl2_core.cuh).
+	 * The default walk in 128-thread blocks only: the other modes and the one-warp variant slice inline. */
+	constexpr bool DEFER = BLOCKED && MODE == 4 && BLOCK == 128;
+	vdl2_defer df;
+	vdl2_defer_init(df);
 	uint32_t m = 0;
 	if(BLOCKED) {
 		if(MODE == 4) {
@@ -1340,6 +1345,9 @@ __device__ __forceinline__ void k2_sync_body(const vdl2_k2_params &p) {
 			for(; m + VDL2_WALK_BLOCK <= n_dec; m += VDL2_WALK_BLOCK, b ^= 1u) {
 				k2_cp_async_wait_all();
 				if(m + 2 * VDL2_WALK_BLOCK <= n_dec) stage(b ^ 1u, (size_t)(m + VDL2_WALK_BLOCK) * s);
+				if(DEFER && vdl2_defer_block<true>(df, v, ring, BLOCK, env, chan, dec_base + m, (int)m, (int)n_dec,
+						&s_sd[b][0][tid], &s_st[b][0][tid], BLOCK, dec, phs, s))
+					continue;
 				vdl2_walk_pref pf;
 				const int first = vdl2_walk_first(v);
 #pragma unroll
@@ -1431,10 +1439,16 @@ __device__ __forceinline__ void k2_sync_body(const vdl2_k2_params &p) {
 	}
 #pragma unroll 1
 	for(; m < n_dec; m++) {
+		if(DEFER) {
+			const int next = vdl2_defer_sample(df, v, env, chan, (int)m, (int)n_dec, dec, phs, s);
+			if(next >= 0) { m = (uint32_t)next - 1u; continue; }
+		}
 		const size_t o = (size_t)m * s;
 		const float2 d = __ldg(&dec[o]);
 		vdl2_demod_step_pm(v, ring, BLOCK, env, chan, dec_base + m, d.x, d.y, __ldg(&phs[o]), MODE == 4 ? vdl2_mag_of(d.x, d.y) : __ldg(&mgs[o]), false, 0.f, 0.f);
 	}
+	/* the data symbols the walk skipped, for all lanes of the warp together */
+	if(DEFER) vdl2_defer_finish(df, v, env, chan, dec, phs, s, (int)n_dec);
 
 #pragma unroll 4
 	for(int i = 0; i < VDL2_SYNC_BUFLEN; i++) p.ring[(size_t)i * s + ch] = ring[i * BLOCK];

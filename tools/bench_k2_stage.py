@@ -9,7 +9,10 @@ The pipelined period is K2a plus the longer of K1 and K2 (+K3) when the overlap 
 sum from the serialised times beside the measured period.  The GPU name, SM clock and power limit are read by NVML in
 the same run.
 
-    python tools/bench_k2_stage.py [--channels 16384] [--chunks 48] [--warmup 8] > k2_stage.json
+--order replica lays the 256 replicas of a slot side by side, so the 32 lanes of a warp carry one signal and never
+diverge; set against the default interleaved order it shows what divergence between lanes costs each kernel.
+
+    python tools/bench_k2_stage.py [--channels 16384] [--order interleaved|replica] [--chunks 48] [--warmup 8] > k2_stage.json
 """
 import argparse
 import json
@@ -29,6 +32,7 @@ def main():
     ap.add_argument("--channels", type=int, default=16384)
     ap.add_argument("--chunks", type=int, default=48, help="timed launches per measurement")
     ap.add_argument("--warmup", type=int, default=8)
+    ap.add_argument("--order", default="interleaved", choices=["interleaved", "replica"], help="channel order, as bench.py --channel-order")
     ap.add_argument("--label", default="", help="free text copied into the result (e.g. which build)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -36,7 +40,7 @@ def main():
     chunks, offs, _ = bench.make_stream(2.0)
     d_chunks = torch.from_numpy(chunks).cuda()
     n_chunks = d_chunks.shape[0]
-    freqs = bench.channel_freqs(offs, a.channels, "interleaved")
+    freqs = bench.channel_freqs(offs, a.channels, a.order)
     stream = torch.cuda.current_stream()
 
     def make(flags):
@@ -46,7 +50,7 @@ def main():
     def feed(g, k):
         g.submit_device(d_chunks[k % n_chunks].data_ptr(), bench.CHUNK_BYTES, stream.cuda_stream)
 
-    res = dict(gpu=torch.cuda.get_device_name(), label=a.label, channels=a.channels, chunk_pairs=bench.CHUNK_PAIRS,
+    res = dict(gpu=torch.cuda.get_device_name(), label=a.label, order=a.order, channels=a.channels, chunk_pairs=bench.CHUNK_PAIRS,
                timed_chunks=a.chunks)
 
     g = make(vd.FLAG_NO_OVERLAP)
