@@ -47,6 +47,73 @@ static const uint16_t *crc_table() {
 	return tab;
 }
 
+/* One launch of n samples of one channel in one of the kernels' walk forms (use_pre: 0 the per-sample walk; 1 blocked on the
+ * phase plane, TwoSum unwrap; 2 the same, table unwrap; 3 the ring walk, inputs requested one block ahead; 4 the staged ring
+ * walk (MODE 3); 5 the default walk (MODE 4), data symbols sliced inline).  dec / phs / mgs: the channel's sample 0 of the
+ * launch in the decimated, phase and magnitude planes, consecutive samples n_ch apart; phs[-k * n_ch] is valid for k <= 160. */
+static void hostsim_walk_launch(int use_pre, vdl2_chan &v, float *ring, const vdl2_k2_env &env, uint32_t ch, uint64_t base, uint32_t n,
+		size_t n_ch, const float2x *dec, const float *phs, const float *mgs) {
+	uint32_t m = 0;
+	if(use_pre == 4) {                /* the kernel's staged ring walk (MODE 3): same control flow, the cp.async copies done at once */
+		float stage[2][16];
+		int first_cur = 0;
+		uint32_t b = 0;
+		if(m + VDL2_WALK_BLOCK <= n) {
+			const int f0 = vdl2_walk_first(v);
+			for(int t = 0; t < VDL2_WALK_BLOCK; t++) stage[0][t] = phs[(size_t)t * n_ch];
+			for(int j = 0; j < 4; j++) stage[0][12 + j] = mgs[(size_t)(f0 + VDL2_SYNC_SKIP * j) * n_ch];
+			first_cur = f0;
+		}
+		for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK, b ^= 1u) {
+			const size_t o = (size_t)m * n_ch;
+			vdl2_walk_pref pf;
+			for(int t = 0; t < VDL2_WALK_BLOCK; t++) pf.pw[t] = stage[b][t];
+			for(int j = 0; j < 4; j++) pf.mg[j] = stage[b][12 + j];
+			pf.first = first_cur; pf.valid = 1;
+			if(m + 2 * VDL2_WALK_BLOCK <= n) {
+				const int fn = vdl2_walk_first(v);
+				const float *ph_n = phs + o + (size_t)VDL2_WALK_BLOCK * n_ch, *mg_n = mgs + o + (size_t)VDL2_WALK_BLOCK * n_ch;
+				for(int t = 0; t < VDL2_WALK_BLOCK; t++) stage[b ^ 1u][t] = ph_n[(size_t)t * n_ch];
+				for(int j = 0; j < 4; j++) stage[b ^ 1u][12 + j] = mg_n[(size_t)(fn + VDL2_SYNC_SKIP * j) * n_ch];
+				first_cur = fn;
+			}
+			vdl2_walk_block_ring(v, ring, 1, env, ch, base + m, dec + o, phs + o, mgs + o, n_ch, pf, false);
+		}
+	} else if(use_pre == 5) {         /* the kernel's default walk (MODE 4): no magnitude plane, the four attempt magnitudes from the samples */
+		for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK) {
+			const size_t o = (size_t)m * n_ch;
+			vdl2_walk_pref pf;
+			const int first = vdl2_walk_first(v);
+			for(int t = 0; t < VDL2_WALK_BLOCK; t++) pf.pw[t] = phs[o + (size_t)t * n_ch];
+			for(int j = 0; j < 4; j++) {
+				const float2x d = dec[o + (size_t)(first + VDL2_SYNC_SKIP * j) * n_ch];
+				pf.mg[j] = vdl2_mag_of(d.x, d.y);
+			}
+			pf.first = first; pf.valid = 1;
+			vdl2_walk_block_ring(v, ring, 1, env, ch, base + m, dec + o, phs + o, nullptr, n_ch, pf, false);
+		}
+	} else if(use_pre == 3) {         /* the kernel's ring walk, inputs requested one block ahead */
+		vdl2_walk_pref pf;
+		memset(&pf, 0, sizeof(pf));
+		for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK) {
+			const size_t o = (size_t)m * n_ch;
+			vdl2_walk_block_ring(v, ring, 1, env, ch, base + m, dec + o, phs + o, mgs + o, n_ch, pf, m + 2 * VDL2_WALK_BLOCK <= n);
+		}
+	} else if(use_pre) {              /* the kernel's blocked walk on the phase plane */
+		for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK) {
+			const size_t o = (size_t)m * n_ch;
+			if(use_pre == 2)              /* unwrap through the transition table */
+				vdl2_walk_block<true>(v, ring, 1, env, ch, base + m, dec + o, phs + o, mgs + o, n_ch);
+			else
+				vdl2_walk_block<false>(v, ring, 1, env, ch, base + m, dec + o, phs + o, mgs + o, n_ch);
+		}
+	}
+	for(; m < n; m++) {
+		const size_t o = (size_t)m * n_ch;
+		vdl2_demod_step_pm(v, ring, 1, env, ch, base + m, dec[o].x, dec[o].y, phs[o], mgs[o], false, 0.f, 0.f);
+	}
+}
+
 extern "C" {
 
 /* K1 restated on the host exactly as the scalar kernel does it (table form of the NCO) */
@@ -130,76 +197,9 @@ int hostsim_k2k3(const float *dec /*[n_dec][n_ch][2]*/, uint32_t n_dec, uint32_t
 		const uint32_t len = launches && n_launches ? launches[li % n_launches] : 1024u;
 		uint32_t n = n_dec - base < len ? n_dec - base : len;
 		for(uint32_t ch = 0; ch < n_ch; ch++) {
-			uint32_t m = 0;
-			if(use_pre == 4) {                /* the kernel's staged ring walk (MODE 3): same control flow, the cp.async copies done at once */
-				float stage[2][16];
-				int first_cur = 0;
-				uint32_t b = 0;
-				const float *phs = &phase[((size_t)base + VDL2_SYNC_BUFLEN) * n_ch + ch];
-				const float *mgs = &mag[(size_t)base * n_ch + ch];
-				if(m + VDL2_WALK_BLOCK <= n) {
-					const int f0 = vdl2_walk_first(chans[ch]);
-					for(int t = 0; t < VDL2_WALK_BLOCK; t++) stage[0][t] = phs[(size_t)t * n_ch];
-					for(int j = 0; j < 4; j++) stage[0][12 + j] = mgs[(size_t)(f0 + VDL2_SYNC_SKIP * j) * n_ch];
-					first_cur = f0;
-				}
-				for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK, b ^= 1u) {
-					const size_t o = (size_t)(base + m) * n_ch + ch;
-					vdl2_walk_pref pf;
-					for(int t = 0; t < VDL2_WALK_BLOCK; t++) pf.pw[t] = stage[b][t];
-					for(int j = 0; j < 4; j++) pf.mg[j] = stage[b][12 + j];
-					pf.first = first_cur; pf.valid = 1;
-					if(m + 2 * VDL2_WALK_BLOCK <= n) {
-						const int fn = vdl2_walk_first(chans[ch]);
-						const float *ph_n = phs + (size_t)(m + VDL2_WALK_BLOCK) * n_ch, *mg_n = mgs + (size_t)(m + VDL2_WALK_BLOCK) * n_ch;
-						for(int t = 0; t < VDL2_WALK_BLOCK; t++) stage[b ^ 1u][t] = ph_n[(size_t)t * n_ch];
-						for(int j = 0; j < 4; j++) stage[b ^ 1u][12 + j] = mg_n[(size_t)(fn + VDL2_SYNC_SKIP * j) * n_ch];
-						first_cur = fn;
-					}
-					vdl2_walk_block_ring(chans[ch], &rings[(size_t)ch * VDL2_SYNC_BUFLEN], 1, env, ch, base + m,
-							reinterpret_cast<const float2 *>(dec2 + o), &phase[o + (size_t)VDL2_SYNC_BUFLEN * n_ch], &mag[o], n_ch, pf, false);
-				}
-			} else if(use_pre == 5) {         /* the kernel's default walk (MODE 4): no magnitude plane, the four attempt magnitudes from the samples */
-				const float *phs = &phase[((size_t)base + VDL2_SYNC_BUFLEN) * n_ch + ch];
-				for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK) {
-					const size_t o = (size_t)(base + m) * n_ch + ch;
-					vdl2_walk_pref pf;
-					const int first = vdl2_walk_first(chans[ch]);
-					for(int t = 0; t < VDL2_WALK_BLOCK; t++) pf.pw[t] = phs[(size_t)(m + t) * n_ch];
-					for(int j = 0; j < 4; j++) {
-						const float *d = &dec[(o + (size_t)(first + VDL2_SYNC_SKIP * j) * n_ch) * 2];
-						pf.mg[j] = vdl2_mag_of(d[0], d[1]);
-					}
-					pf.first = first; pf.valid = 1;
-					vdl2_walk_block_ring(chans[ch], &rings[(size_t)ch * VDL2_SYNC_BUFLEN], 1, env, ch, base + m,
-							reinterpret_cast<const float2 *>(dec2 + o), &phase[o + (size_t)VDL2_SYNC_BUFLEN * n_ch], nullptr, n_ch, pf, false);
-				}
-			} else if(use_pre == 3) {         /* the kernel's ring walk, inputs requested one block ahead */
-				vdl2_walk_pref pf;
-				memset(&pf, 0, sizeof(pf));
-				for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK) {
-					const size_t o = (size_t)(base + m) * n_ch + ch;
-					vdl2_walk_block_ring(chans[ch], &rings[(size_t)ch * VDL2_SYNC_BUFLEN], 1, env, ch, base + m,
-							reinterpret_cast<const float2 *>(dec2 + o), &phase[o + (size_t)VDL2_SYNC_BUFLEN * n_ch], &mag[o], n_ch,
-							pf, m + 2 * VDL2_WALK_BLOCK <= n);
-				}
-			} else if(use_pre) {              /* the kernel's blocked walk on the phase plane */
-				for(; m + VDL2_WALK_BLOCK <= n; m += VDL2_WALK_BLOCK) {
-					const size_t o = (size_t)(base + m) * n_ch + ch;
-					if(use_pre == 2)              /* unwrap through the transition table */
-						vdl2_walk_block<true>(chans[ch], &rings[(size_t)ch * VDL2_SYNC_BUFLEN], 1, env, ch, base + m,
-								reinterpret_cast<const float2 *>(dec2 + o), &phase[o + (size_t)VDL2_SYNC_BUFLEN * n_ch], &mag[o], n_ch);
-					else
-						vdl2_walk_block<false>(chans[ch], &rings[(size_t)ch * VDL2_SYNC_BUFLEN], 1, env, ch, base + m,
-								reinterpret_cast<const float2 *>(dec2 + o), &phase[o + (size_t)VDL2_SYNC_BUFLEN * n_ch], &mag[o], n_ch);
-				}
-			}
-			for(; m < n; m++) {
-				const size_t o = (size_t)(base + m) * n_ch + ch;
-				const float *d = &dec[o * 2];
-				vdl2_demod_step_pm(chans[ch], &rings[(size_t)ch * VDL2_SYNC_BUFLEN], 1, env, ch, base + m, d[0], d[1],
-						phase[o + (size_t)VDL2_SYNC_BUFLEN * n_ch], mag[o], false, 0.f, 0.f);
-			}
+			const size_t o = (size_t)base * n_ch + ch;
+			hostsim_walk_launch(use_pre, chans[ch], &rings[(size_t)ch * VDL2_SYNC_BUFLEN], env, ch, base, n, n_ch, dec2 + o,
+					&phase[o + (size_t)VDL2_SYNC_BUFLEN * n_ch], &mag[o]);
 		}
 		for(uint32_t b = 0; b < ctl.n_ready; b++) {
 			const vdl2_burst_slot *slot = &pool[ready[b]];

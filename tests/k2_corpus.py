@@ -482,3 +482,119 @@ def ragged_tail_cells(spans, oracles):
                 key = ({1: "sync", 2: "header", 3: "end"}[e["kind"]], p - BLOCK * (c // BLOCK))
                 cells[key] = cells.get(key, 0) + 1
     return cells, lengths
+
+
+# ---- deferral edges of the ragged walk: the default walk skips a burst's data symbols and slices them after the walk
+# (vdl2_defer), one queued burst per lane.  A second fleet of mostly short one-frame bursts back to back, whose span counts
+# are planned from the oracle's burst ends (kind 3, the sample of a burst's last symbol) so that each receiver cycles
+# through the cases where deferral can go wrong, offset per receiver so that the lanes of a warp are in different ones.
+DEFER_CASES = ("end_on_last_sample",         # a span ends exactly on a burst's last symbol
+               "end_on_next_first_sample",   # ... one sample before it: the last symbol is the next span's first sample
+               "end_on_last_sample_but_one", # ... one sample after it
+               "empty_span_while_open",      # a zero-count span while the burst is open
+               "empty_spans_while_open",     # several in a row
+               "one_sample_spans_in_data",   # a run of one-sample spans inside the burst's data
+               "two_ends_in_a_span",         # a span holding two burst ends: the second finds the queue taken
+               "three_ends_in_a_span")       # ... three
+
+
+@functools.lru_cache(maxsize=None)
+def defer_fleet(n_rx=64, seconds=0.25):
+    """[dict(centre, freqs, os, fmt, buf)]: receiver r has one channel, oversample 10 cu8 or 20 cs16, one-frame bursts of
+    8-24 octets back to back with gaps of 0-50 decimated samples, about one in twelve a long one of 150-250 octets"""
+    out = []
+    for r in range(n_rx):
+        os_, fmt = ((10, "u8"), (20, "s16"))[r % 2]
+        rng = np.random.default_rng(0x444546 + r)
+        off = (0.0, 25e3, -37.5e3)[r % 3]
+        t, bursts = float(rng.uniform(0.0005, 0.003)), []
+        while t < seconds - 0.03:
+            frames = synth.random_frames(rng, 1, 150, 250) if rng.random() < 1 / 12 else synth.random_frames(rng, 1, 8, 24)
+            bursts.append(synth.BurstSpec(t, off, frames, power_dbfs=-14.0))
+            t += synth.burst_duration_s(frames) + float(rng.integers(0, 51)) / DEC_RATE
+        iq = synth.synth_stream(DEC_RATE * os_, seconds, bursts, es_n0_db=30, fmt=fmt, seed=0x4445 + r)
+        centre = 136100000 + 125000 * r
+        out.append(dict(centre=centre, freqs=[centre + int(off)], os=os_, fmt=fmt,
+                        buf=np.ascontiguousarray(iq).view(np.uint8).reshape(-1)))
+    return out
+
+
+@functools.lru_cache(maxsize=None)
+def defer_oracles():
+    """the oracle's run of every receiver of the deferral fleet, trace and decimated-sample tap on"""
+    from oracle import pyoracle as po
+    res = []
+    for x in defer_fleet():
+        o = po.Oracle(DEC_RATE * x["os"], x["os"], po.FMT_S16 if x["fmt"] == "s16" else po.FMT_U8, x["centre"], x["freqs"],
+                      trace=True, dec_tap=True)
+        o.process(x["buf"])
+        res.append(o)
+    return res
+
+
+def defer_counts(n_dec, ends, k0, width=RAGGED_W):
+    """one receiver's span counts: its burst ends take the DEFER_CASES in turn from case k0 on; fillers between them take
+    RAGGED_LENGTHS in turn"""
+    counts, pos, fill = [], 0, k0
+
+    def fill_to(cut):
+        nonlocal pos, fill
+        while pos < cut:
+            f = min(RAGGED_LENGTHS[fill % len(RAGGED_LENGTHS)], cut - pos)
+            counts.append(f)
+            pos += f
+            fill += 1
+
+    def one_span_to(cut, first_end):
+        """fillers, then one span up to cut that holds first_end and the walk after it"""
+        nonlocal pos
+        start = max(pos, cut - width)
+        if start >= first_end:
+            return False
+        fill_to(start)
+        counts.append(cut - pos)
+        pos = cut
+        return True
+
+    ends = sorted(ends)
+    j, case = 0, k0
+    while j < len(ends):
+        e = ends[j]
+        if e < pos + 130:                          # too close to where the plan stands: the next one
+            j += 1
+            continue
+        kind = DEFER_CASES[case % len(DEFER_CASES)]
+        used = 1
+        if kind == "end_on_last_sample":
+            fill_to(e + 1)
+        elif kind == "end_on_next_first_sample":
+            fill_to(e)
+        elif kind == "end_on_last_sample_but_one":
+            fill_to(e + 2)
+        elif kind in ("empty_span_while_open", "empty_spans_while_open"):
+            fill_to(e - 100)
+            counts += [0] * (1 if kind == "empty_span_while_open" else 4)
+        elif kind == "one_sample_spans_in_data":
+            fill_to(e - 60)
+            counts += [1] * 12
+            pos += 12
+        else:
+            used = 2 if kind == "two_ends_in_a_span" else 3
+            if j + used - 1 >= len(ends) or not one_span_to(ends[j + used - 1] + 5, e):
+                j += 1
+                continue
+        j += used
+        case += 1
+    while pos < n_dec:
+        f = min(width, n_dec - pos)
+        counts.append(f)
+        pos += f
+    return counts
+
+
+def defer_spans(oracles, n_dec):
+    """[span][receiver] counts of the deferral fleet (0 when a receiver's plan has run out of spans)"""
+    per = [defer_counts(n_dec[r], [int(e["dec_index"]) for e in o.events() if e["kind"] == 3], 3 * r)
+           for r, o in enumerate(oracles)]
+    n_spans = max(len(c) for c in per)
+    return [[c[s] if s < len(c) else 0 for c in per] for s in range(n_spans)]

@@ -15,7 +15,10 @@ from tests import k2_corpus as kc
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "..", "dumpvdl2_b200", "csrc")
 STATS = ["end_at_block_offset_%d" % k for k in range(12)] + ["end_in_tail", "queued", "sliced_at_once", "no_pool_slot",
-                                                              "open_completed_on_last_sample"]
+                                                              "open_completed_on_last_sample", "end_on_last_sample_but_one",
+                                                              "last_symbol_on_next_first_sample", "two_ends_in_a_launch",
+                                                              "three_ends_in_a_launch", "open_across_an_empty_span",
+                                                              "one_sample_span_in_data"]
 
 # (stage, channels, launch schedule, pool slots or None for the usual 3 per channel + 16)
 CASES = {
@@ -40,8 +43,9 @@ def lib(tmp_path_factory):
     subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-w",
                            "-I", CSRC, "-o", so, os.path.join(HERE, "hostsim", "defer.cpp")])
     L = C.CDLL(so)
-    L.hostsim_k2_defer_check.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_float, C.c_uint32,
-                                         C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    for f in (L.hostsim_k2_defer_check, L.hostsim_k2_defer_check_spans):
+        f.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_float, C.c_uint32, C.c_void_p, C.c_uint32,
+                      C.c_void_p, C.c_void_p]
     return L
 
 
@@ -72,11 +76,34 @@ def test_deferred_data_symbols_leave_every_launch_as_the_inline_walk(lib, case):
 
 
 def test_deferred_walk_reaches_its_own_cases(lib):
-    """the cases above hit every way a deferred burst can end"""
+    """the cases above hit every way a deferred burst can end (an empty span takes per-receiver spans, below)"""
     total = {}
     for case in CASES:
         for k, v in _run(lib, case)[2].items():
             total[k] = total.get(k, 0) + v
     print(total)
-    empty = [k for k, v in total.items() if v == 0]
+    empty = [k for k, v in total.items() if v == 0 and k != "open_across_an_empty_span"]
+    assert not empty, f"not reached: {empty}"
+
+
+def test_ragged_deferral_plan_leaves_every_span_as_the_inline_walk_and_reaches_every_cell(lib):
+    """k2_corpus.defer_spans: 64 one-receiver channels, each on its own span counts (zeros included), planned from the
+    oracle's burst ends so that spans end on, one before and one after a burst's last symbol, come empty or one sample
+    long while a burst is open, and hold two and three burst ends.  After every span the deferred walk leaves what the
+    inline walk leaves, and every cell of the plan is reached."""
+    oracles = kc.defer_oracles()
+    dec = np.ascontiguousarray(np.concatenate([o.dec_samples() for o in oracles], axis=1), np.float32)
+    freqs = np.ascontiguousarray([x["freqs"][0] for x in kc.defer_fleet()], np.uint32)
+    spans = np.ascontiguousarray(kc.defer_spans(oracles, [dec.shape[0]] * dec.shape[1]), np.uint32)
+    stats = np.zeros(len(STATS), np.uint64)
+    bad_ch = C.c_int32(-1)
+    bad = lib.hostsim_k2_defer_check_spans(dec.ctypes.data, dec.shape[0], dec.shape[1], freqs.ctypes.data, 2100000, 0.0,
+                                           3 * dec.shape[1] + 16, spans.ctypes.data, spans.shape[0], stats.ctypes.data,
+                                           C.byref(bad_ch))
+    cells = dict(zip(STATS, (int(x) for x in stats)))
+    for k, v in cells.items():
+        print(f"{k:40s} {v}")
+    assert bad == -1, f"span {bad} differs (channel {bad_ch.value})"
+    assert (spans == 0).any() and (spans == 1).any()
+    empty = [k for k, v in cells.items() if v == 0 and k != "no_pool_slot"]
     assert not empty, f"not reached: {empty}"
