@@ -17,6 +17,8 @@ FMT_U8, FMT_S16 = 0, 1
 FLAG_TRACE, FLAG_KEEP_DEC, FLAG_K1_SCALAR, FLAG_NO_OVERLAP, FLAG_NO_GRAPH, FLAG_RAGGED = 1, 2, 4, 8, 16, 32
 FLAG_INPUT_LEVELS = 64
 FLAG_CHANNEL_LEVELS = 128
+FLAG_SPECTRUM = 256
+SPECTRUM_BINS = 1024
 CHANNEL_LEVEL_BINS = 40
 NUM_COUNTERS = 9
 COUNTER_NAMES = ["sync_good", "hdr_crc_good", "bursts", "burst_err", "blocks_processed",
@@ -72,6 +74,11 @@ class _ChannelLevels(C.Structure):
                 ("mag_lp", C.c_float), ("mag_nf", C.c_float), ("nf_pwr_dbfs", C.c_float)]
 
 
+class _Spectrum(C.Structure):
+    _fields_ = [("segments", C.c_uint64), ("pending", C.c_uint32), ("reserved", C.c_uint32), ("pow_lo", C.c_uint64 * SPECTRUM_BINS),
+                ("pow_hi", C.c_uint64 * SPECTRUM_BINS), ("peak", C.c_float * SPECTRUM_BINS)]
+
+
 class _Event(C.Structure):
     _fields_ = [("channel", C.c_uint32), ("kind", C.c_uint32), ("dec_index", C.c_uint64),
                 ("i", C.c_int32 * 8), ("f", C.c_float * 8)]
@@ -121,6 +128,7 @@ def load_library():
     L.vdl2gpu_get_channel_counters.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.vdl2gpu_get_input_levels.argtypes = [C.c_void_p, C.POINTER(_InputLevels), C.c_uint32]
     L.vdl2gpu_get_channel_levels.argtypes = [C.c_void_p, C.POINTER(_ChannelLevels), C.c_uint32]
+    L.vdl2gpu_get_spectrum.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.POINTER(_Spectrum)]
     L.vdl2gpu_get_tables.argtypes = [C.c_void_p] + [C.c_void_p] * 8
     L.vdl2gpu_read_dec.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]
     L.vdl2gpu_read_events.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
@@ -230,6 +238,23 @@ def channel_level_metrics(rec):
                 peak_dbfs=10.0 * np.log10(pk) if pk > 0 else float("-inf"), nf_dbfs=float(rec["nf_pwr_dbfs"]), bin_floor_dbfs=edges)
 
 
+def spectrum_metrics(rec, centerfreq, sample_rate):
+    """What an operator reads off one record of spectrum(), for an input tuned to centerfreq at sample_rate (Hz): freq_hz,
+    the frequency of each bin; mean_dbfs, the mean power per bin, 10 log10(pow / 2^40 / segments / 512^2), so that a
+    full-scale complex tone on a bin reads 0 dBFS (-inf for a bin that only saw silence); peak_dbfs, the peak hold on the
+    same scale.  The powers are None for an input that has no complete segment yet."""
+    n = SPECTRUM_BINS
+    freq = float(centerfreq) + (np.arange(n, dtype=np.float64) - n // 2) * (float(sample_rate) / n)
+    segs = int(rec["segments"])
+    if segs == 0:
+        return dict(freq_hz=freq, mean_dbfs=None, peak_dbfs=None)
+    full = float(n // 2) ** 2                        # sum of the Hann window, squared
+    mean = np.array([int(v) for v in rec["pow"]], dtype=np.float64) / float(1 << 40) / segs / full
+    peak = np.asarray(rec["peak"], np.float64) / full
+    with np.errstate(divide="ignore"):
+        return dict(freq_hz=freq, mean_dbfs=10.0 * np.log10(mean), peak_dbfs=10.0 * np.log10(peak))
+
+
 def make_config(sample_rate, oversample, sample_fmt, centerfreq, freqs, max_ppm=0.0, flags=0):
     """(vdl2gpu_config, the freqs array it points at) for the stage stubs"""
     fr = np.ascontiguousarray(freqs, dtype=np.uint32)
@@ -255,14 +280,18 @@ class Vdl2Channels:
     """N VDL2 channels demodulated from one IQ stream on one H100."""
 
     def __init__(self, sample_rate, oversample, sample_fmt, centerfreq, freqs, max_ppm=0.0,
-                 max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, n_streams=1, levels=False, channel_levels=False):
+                 max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, n_streams=1, levels=False, channel_levels=False,
+                 spectrum=False):
         """n_streams > 1: independent-streams mode, channels [s*C, (s+1)*C) demodulate stream s; process_buf_* then take
         the S per-stream buffers back to back.  levels=True: measure every input's levels (input_levels());
-        channel_levels=True: measure every channel's in-band levels (channel_levels())."""
+        channel_levels=True: measure every channel's in-band levels (channel_levels()); spectrum=True: measure every
+        input's power spectrum (spectrum())."""
         if levels:
             flags |= FLAG_INPUT_LEVELS
         if channel_levels:
             flags |= FLAG_CHANNEL_LEVELS
+        if spectrum:
+            flags |= FLAG_SPECTRUM
         self.L = load_library()
         self.n_streams = int(n_streams)
         self.freqs = np.ascontiguousarray(freqs, dtype=np.uint32)
@@ -421,6 +450,24 @@ class Vdl2Channels:
         return [dict(hist=np.array(o.hist[:], np.uint64), pow=(o.pow_hi << 64) | o.pow_lo, peak_pow=np.float32(o.peak_pow),
                      mag_lp=np.float32(o.mag_lp), mag_nf=np.float32(o.mag_nf), nf_pwr_dbfs=np.float32(o.nf_pwr_dbfs)) for o in out[:n]]
 
+    def spectrum(self, first=0, n=None):
+        """one dict per input first .. first + n - 1 (default: to the last input; inputs as for input_levels()) of what the
+        device measured over every complete 1024-sample segment so far: segments, pending (samples of the incomplete segment
+        held), pow (object array of 1024 Python ints, the 128-bit sums of p x 2^40 per bin) and peak (float32 array of the
+        largest p per bin).  Bin k is centre + (k - 512) fs / 1024 (see vdl2gpu_get_spectrum; spectrum_metrics() turns one
+        into Hz and dBFS).  Needs spectrum=True at creation."""
+        if n is None:
+            n = max(self.n_streams - first, 0)
+        out = (_Spectrum * max(n, 1))()
+        _check(self.L, self.L.vdl2gpu_get_spectrum(self.h, first, n, out), "vdl2gpu_get_spectrum")
+        recs = []
+        for o in out[:n]:
+            lo = np.ctypeslib.as_array(o.pow_lo).astype(object)
+            hi = np.ctypeslib.as_array(o.pow_hi).astype(object)
+            recs.append(dict(segments=o.segments, pending=o.pending, pow=(hi << 64) | lo,
+                             peak=np.ctypeslib.as_array(o.peak).astype(np.float32).copy()))
+        return recs
+
     def kernel_ms(self):
         ms = (C.c_double * 5)()
         n = (C.c_uint64 * 5)()
@@ -434,13 +481,15 @@ class Vdl2Receivers(Vdl2Channels):
     channels_of(r).  The receivers advance in lock step: submit() takes one equal-length buffer per receiver."""
 
     def __init__(self, sample_rate, oversample, sample_fmt, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1,
-                 flags=0, n_inflight=4, levels=False, channel_levels=False):
+                 flags=0, n_inflight=4, levels=False, channel_levels=False, spectrum=False):
         """receivers: list of (centerfreq, [channel freqs...]); levels=True: measure every receiver's input levels;
-        channel_levels=True: every channel's in-band levels"""
+        channel_levels=True: every channel's in-band levels; spectrum=True: every receiver's power spectrum"""
         if levels:
             flags |= FLAG_INPUT_LEVELS
         if channel_levels:
             flags |= FLAG_CHANNEL_LEVELS
+        if spectrum:
+            flags |= FLAG_SPECTRUM
         self.L = load_library()
         self.receivers = [(int(cf), [int(f) for f in fr]) for cf, fr in receivers]
         self.n_receivers = self.n_streams = len(self.receivers)
@@ -503,16 +552,18 @@ class Vdl2MixedReceivers(Vdl2Receivers):
     remove_receivers() let receivers join and leave (after flush()) while the others carry on."""
 
     def __init__(self, receivers, max_ppm=0.0, max_chunk_bytes=1 << 20, device=-1, flags=0, n_inflight=4, ragged=False,
-                 levels=False, channel_levels=False):
+                 levels=False, channel_levels=False, spectrum=False):
         """receivers: list of (centerfreq, [channel freqs...], oversample (10, 13 or 20), fmt (FMT_U8 or FMT_S16));
         levels=True: measure every receiver's input levels (input_levels()); channel_levels=True: every channel's in-band
-        levels (channel_levels())"""
+        levels (channel_levels()); spectrum=True: every receiver's power spectrum (spectrum())"""
         if ragged:
             flags |= FLAG_RAGGED
         if levels:
             flags |= FLAG_INPUT_LEVELS
         if channel_levels:
             flags |= FLAG_CHANNEL_LEVELS
+        if spectrum:
+            flags |= FLAG_SPECTRUM
         self.ragged = bool(flags & FLAG_RAGGED)
         self.L = load_library()
         rxs = self._normalise(receivers)

@@ -1703,4 +1703,108 @@ VDL2_HD uint64_t vdl2_chlv_q(float p) {
 #endif
 }
 
+/* ------------------------------------------------------------------------------------------------
+ * Spectrum (VDL2GPU_FLAG_SPECTRUM): the power spectrum of every input in VDL2_SPEC_N bins.  Segment j of an input is its
+ * complex samples [N j, N (j + 1)) counted from the grid's origin (create, the receiver's joining, its restart), x_n the
+ * float K0 made of sample n.  Per segment: y_n = fl32(x_n w_n) with the periodic Hann window w; a radix-2 decimation-in-time
+ * FFT over the bit-reversed y, every product and sum rounded on its own; the power of each bin p = fl32(fl32(re re) +
+ * fl32(im im)) (vdl2_chlv_pow), stored shifted: stored bin k holds FFT bin (k + N/2) mod N, frequency (k - N/2) fs / N.
+ * Per input and stored bin, cumulative: the 128-bit sum of q = (uint64)(p 2^40) and the largest p.
+ * |X_k| <= sum of w |x| <= 512 sqrt(2), so p <= 2^19 and q < 2^60.
+ * ---------------------------------------------------------------------------------------------- */
+#define VDL2_SPEC_N 1024u
+#define VDL2_SPEC_LOG2N 10u
+
+/* per input, in device memory: the accumulators (lo, hi: q sums; peak: p's float bits, p >= 0 so the bits order like the
+ * values), then the samples of the segment not yet complete (carry[0, pending)) */
+typedef struct {
+	uint64_t lo[VDL2_SPEC_N];
+	uint64_t hi[VDL2_SPEC_N];
+	uint32_t peak[VDL2_SPEC_N];
+	float2 carry[VDL2_SPEC_N];
+} vdl2_spec_acc;
+
+/* the window and the twiddles, made once on the host: w_n = 0.5 - 0.5 cos(2 pi n / N) and W^k = (cos(2 pi k / N),
+ * -sin(2 pi k / N)) for k < N/2, each evaluated in double and rounded to float once */
+typedef struct {
+	float win[VDL2_SPEC_N];
+	float2 tw[VDL2_SPEC_N / 2];
+} vdl2_spec_tab;
+
+static inline void vdl2_spec_make_tab(vdl2_spec_tab *t) {
+	for(uint32_t n = 0; n < VDL2_SPEC_N; n++) t->win[n] = (float)(0.5 - 0.5 * cos(2.0 * VDL2_PI * (double)n / (double)VDL2_SPEC_N));
+	for(uint32_t k = 0; k < VDL2_SPEC_N / 2; k++) {
+		t->tw[k].x = (float)cos(2.0 * VDL2_PI * (double)k / (double)VDL2_SPEC_N);
+		t->tw[k].y = (float)-sin(2.0 * VDL2_PI * (double)k / (double)VDL2_SPEC_N);
+	}
+}
+
+VDL2_HD uint32_t vdl2_spec_bitrev(uint32_t n) {
+	uint32_t r = 0;
+	for(uint32_t b = 0; b < VDL2_SPEC_LOG2N; b++) r |= ((n >> b) & 1u) << (VDL2_SPEC_LOG2N - 1u - b);
+	return r;
+}
+VDL2_HD float2 vdl2_spec_windowed(float2 x, float w) { float2 y; y.x = F_MUL(x.x, w); y.y = F_MUL(x.y, w); return y; }
+/* butterfly b (< N/2) of stage s (0 .. LOG2N - 1): the pair it combines and the twiddle it takes */
+VDL2_HD void vdl2_spec_pair(uint32_t s, uint32_t b, uint32_t &i0, uint32_t &i1, uint32_t &k) {
+	const uint32_t half = 1u << s, j = b & (half - 1u);
+	i0 = ((b >> s) << (s + 1u)) + j;
+	i1 = i0 + half;
+	k = j << (VDL2_SPEC_LOG2N - 1u - s);
+}
+/* a, b <- a + w b, a - w b */
+VDL2_HD void vdl2_spec_bfly(float2 &a, float2 &b, float2 w) {
+	const float tr = F_SUB(F_MUL(b.x, w.x), F_MUL(b.y, w.y));
+	const float ti = F_ADD(F_MUL(b.x, w.y), F_MUL(b.y, w.x));
+	b.x = F_SUB(a.x, tr); b.y = F_SUB(a.y, ti);
+	a.x = F_ADD(a.x, tr); a.y = F_ADD(a.y, ti);
+}
+/* the FFT bin stored bin k holds */
+VDL2_HD uint32_t vdl2_spec_fft_bin(uint32_t k) { return (k + VDL2_SPEC_N / 2u) & (VDL2_SPEC_N - 1u); }
+/* p 2^40 truncated: the scaling is exact and p < 2^20, so q < 2^60 */
+VDL2_HD uint64_t vdl2_spec_q(float p) {
+#if defined(__CUDA_ARCH__)
+	return __float2ull_rz(p * 1099511627776.0f);
+#else
+	return (uint64_t)(p * 1099511627776.0f);
+#endif
+}
+
+/* One segment, serially (the device runs the same butterflies in parallel): x[N] in, p[N] (stored order) out; buf[N] is
+ * scratch */
+VDL2_HD void vdl2_spec_segment(const float2 *x, const vdl2_spec_tab *t, float2 *buf, float *p) {
+	for(uint32_t n = 0; n < VDL2_SPEC_N; n++) buf[vdl2_spec_bitrev(n)] = vdl2_spec_windowed(x[n], t->win[n]);
+	for(uint32_t s = 0; s < VDL2_SPEC_LOG2N; s++)
+		for(uint32_t b = 0; b < VDL2_SPEC_N / 2u; b++) {
+			uint32_t i0, i1, k;
+			vdl2_spec_pair(s, b, i0, i1, k);
+			vdl2_spec_bfly(buf[i0], buf[i1], t->tw[k]);
+		}
+	for(uint32_t k = 0; k < VDL2_SPEC_N; k++) {
+		const float2 v = buf[vdl2_spec_fft_bin(k)];
+		p[k] = vdl2_chlv_pow(v.x, v.y);
+	}
+}
+
+/* The segment grid of one input in one chunk or span: it holds `pend` samples of its incomplete segment (its position
+ * since the grid's origin, mod N) and brings n.  Sample m of the chunk's segment j is the input's sample N j + m - pend of
+ * the chunk when that is >= 0, else carry[pend + (N j + m - pend)]. */
+typedef struct {
+	uint32_t pend, n;
+} vdl2_spec_span;
+
+/* the grid entry of a chunk that brings n samples to an input at position pos (samples since the grid's origin), which
+ * then advances */
+VDL2_HD vdl2_spec_span vdl2_spec_step(uint64_t &pos, uint32_t n) {
+	vdl2_spec_span e;
+	e.pend = (uint32_t)(pos & (VDL2_SPEC_N - 1u));
+	e.n = n;
+	pos += n;
+	return e;
+}
+VDL2_HD uint32_t vdl2_spec_segments(vdl2_spec_span e) { return (uint32_t)(((uint64_t)e.pend + e.n) >> VDL2_SPEC_LOG2N); }
+VDL2_HD uint32_t vdl2_spec_rest(vdl2_spec_span e) { return (e.pend + e.n) & (VDL2_SPEC_N - 1u); }
+/* where sample m of segment j comes from: >= 0 the chunk's sample, < 0 carry[pend + that] */
+VDL2_HD int64_t vdl2_spec_src(vdl2_spec_span e, uint32_t j, uint32_t m) { return (int64_t)j * VDL2_SPEC_N + m - e.pend; }
+
 #endif

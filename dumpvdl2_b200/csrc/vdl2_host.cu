@@ -71,6 +71,9 @@ struct chunk_slot {
 	/* pushed spans (vdl2gpu_submit_pushed): K0 reads the receivers' rings; k0_done is recorded after it (ragged contexts) */
 	bool pushed = false;
 	cudaEvent_t k0_done = nullptr;
+	/* spectrum (VDL2GPU_FLAG_SPECTRUM): per input, the samples it holds and brings to this chunk (pinned host copy, device
+	 * copy made right before the spectrum kernel) */
+	vdl2_spec_span *h_spec = nullptr, *d_spec = nullptr;
 	cudaGraphExec_t g_front[6] = { nullptr }, g_k2a[6] = { nullptr }, g_back[6] = { nullptr };    /* index = chunk number mod 6 (dec buffer, plane) */
 	uint32_t graph_pairs[6] = { 0 };
 	uint64_t first_pair = 0, dec_base = 0;
@@ -192,6 +195,13 @@ struct vdl2gpu_ctx {
 	/* channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS; NULL otherwise): the per-slot planes the levels form of K2a adds every
 	 * decimated sample to, uint64 [VDL2_CHLV_ROWS][n_chp] then the uint32 peak plane [n_chp] */
 	uint64_t *d_chlv = nullptr;
+	/* spectrum (VDL2GPU_FLAG_SPECTRUM; NULL / empty otherwise): per input its accumulators and waiting samples, the window and
+	 * twiddle tables, and per input its position on its segment grid (samples since the grid's origin: create, joining,
+	 * restart); inputs whose figures a restart zeroes at the start of the next span */
+	vdl2_spec_acc *d_spec = nullptr;
+	vdl2_spec_tab *d_spec_tab = nullptr;
+	std::vector<uint64_t> spec_pos;
+	std::vector<uint32_t> spec_zero;
 };
 
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
@@ -244,6 +254,8 @@ static void free_layout(vdl2gpu_ctx *c) {
 		if(s.d_span) cudaFree(s.d_span);
 		if(s.h_restart) cudaFreeHost(s.h_restart);
 		if(s.d_restart) cudaFree(s.d_restart);
+		if(s.h_spec) cudaFreeHost(s.h_spec);
+		if(s.d_spec) cudaFree(s.d_spec);
 	}
 	c->chunks.clear();
 	cudaFree(c->d_samples);
@@ -254,6 +266,7 @@ static void free_layout(vdl2gpu_ctx *c) {
 	cudaFree(c->d_slot_rx); cudaFree(c->d_block_rx);
 	cudaFree(c->d_rx_in); cudaFree(c->d_slot_cls);
 	cudaFree(c->d_levels); cudaFree(c->d_chlv);
+	cudaFree(c->d_spec); cudaFree(c->d_spec_tab);
 }
 
 /* the pushed-input rings and their queues (no push, copy or span may be running on them) */
@@ -437,6 +450,16 @@ static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu
 		CU(cudaMalloc(&c->d_chlv, bytes));
 		CU(cudaMemset(c->d_chlv, 0, bytes));
 	}
+	if(c->cfg.flags & VDL2GPU_FLAG_SPECTRUM) {
+		CU(cudaMalloc(&c->d_spec, (size_t)c->n_streams * sizeof(vdl2_spec_acc)));
+		CU(cudaMemset(c->d_spec, 0, (size_t)c->n_streams * sizeof(vdl2_spec_acc)));
+		std::unique_ptr<vdl2_spec_tab> tab(new vdl2_spec_tab);
+		vdl2_spec_make_tab(tab.get());
+		CU(cudaMalloc(&c->d_spec_tab, sizeof(vdl2_spec_tab)));
+		CU(cudaMemcpy(c->d_spec_tab, tab.get(), sizeof(vdl2_spec_tab), cudaMemcpyHostToDevice));
+		c->spec_pos.assign(c->n_streams, 0);
+		c->spec_zero.clear();
+	}
 	if(c->mixed) {
 		CU(cudaMalloc(&c->d_rx_in, c->rx_in.size() * sizeof(vdl2_rx_input)));
 		CU(cudaMalloc(&c->d_slot_cls, slot_cls.size()));
@@ -459,6 +482,10 @@ static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu
 		}
 		CU(cudaHostAlloc((void **)&s.h_out, sizeof(vdl2_out_header) + c->out_cap, cudaHostAllocMapped));
 		CU(cudaHostGetDevicePointer((void **)&s.d_out, s.h_out, 0));
+		if(c->d_spec) {
+			CU(cudaHostAlloc((void **)&s.h_spec, (size_t)c->n_streams * sizeof(vdl2_spec_span), cudaHostAllocDefault));
+			CU(cudaMalloc(&s.d_spec, (size_t)c->n_streams * sizeof(vdl2_spec_span)));
+		}
 		memset(s.h_out, 0, sizeof(vdl2_out_header));
 		CU(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
 		for(auto &ev : s.tk) CU(cudaEventCreate(&ev));
@@ -487,6 +514,7 @@ static void swap_layout(vdl2gpu_ctx *a, vdl2gpu_ctx *b) {
 	swap(a->d_k1, b->d_k1); swap(a->d_k2, b->d_k2); swap(a->d_counters, b->d_counters); swap(a->d_ring, b->d_ring);
 	swap(a->d_pool, b->d_pool); swap(a->d_free, b->d_free); swap(a->d_ready, b->d_ready); swap(a->d_ctl, b->d_ctl);
 	swap(a->d_levels, b->d_levels); swap(a->d_chlv, b->d_chlv);
+	swap(a->d_spec, b->d_spec); swap(a->d_spec_tab, b->d_spec_tab); swap(a->spec_pos, b->spec_pos); swap(a->spec_zero, b->spec_zero);
 	swap(a->chunks, b->chunks);
 }
 
@@ -965,6 +993,25 @@ static int launch_k0_span(vdl2gpu_ctx *c, const chunk_slot &s, const void *d_raw
 	return VDL2GPU_OK;
 }
 
+/* Spectrum of the chunk just converted: it reads the sample plane after K0 and before the next chunk's K0 rewrites it, in
+ * the front stream's own order, behind K1.  There it runs while K2 of the previous chunk still holds its one block per SM,
+ * and before K2a, so the lock step of K2 and K1 launched together into an empty machine after K2a is left as it was. */
+static int launch_spectrum(vdl2gpu_ctx *c, chunk_slot &s, uint32_t n_pairs) {
+	CU(cudaMemcpyAsync(s.d_spec, s.h_spec, c->n_streams * sizeof(vdl2_spec_span), cudaMemcpyHostToDevice, c->stream));
+	KL(vdl2_launch_spectrum(reinterpret_cast<const float *>(c->d_samples), c->mixed ? n_pairs * c->rx_os_max : n_pairs, c->n_streams,
+			c->lane_streams ? c->n_chp : c->max_pairs, c->lane_streams ? c->lanes : 0u, c->full_warps, s.d_spec, c->d_spec_tab, c->d_spec,
+			c->stream));
+	return VDL2GPU_OK;
+}
+
+/* every input's entry of the chunk's segment grid (the samples K0 puts in its row or column), its position advanced */
+static void fill_spectrum(vdl2gpu_ctx *c, chunk_slot &s, uint32_t n_pairs) {
+	for(uint32_t i = 0; i < c->n_streams; i++) {
+		const uint32_t n = c->ragged ? s.h_span[i].n * c->rx_in[i].oversample : c->mixed ? n_pairs * c->rx_in[i].oversample : n_pairs;
+		s.h_spec[i] = vdl2_spec_step(c->spec_pos[i], n);
+	}
+}
+
 struct capture_env { vdl2gpu_ctx *c; chunk_slot *s; uint64_t seq; uint32_t n_pairs; uint32_t k0_fmt; };
 #define CAPTURE_PARAMS \
 	capture_env *e = static_cast<capture_env *>(a); \
@@ -985,6 +1032,7 @@ static int body_front(void *a) {
 	else KL(vdl2_launch_k0(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
 			e->n_pairs * bpp, c->max_pairs, e->s->d_args, c->d_levels, c->stream));
 	KL(vdl2_launch_k1(&p1, (c->cfg.flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->stream));
+	if(c->d_spec) { int rc = launch_spectrum(c, *e->s, e->n_pairs); if(rc) return rc; }
 	return 0;
 }
 static int body_k2a(void *a) {
@@ -1038,6 +1086,7 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	if(graph && ensure_graphs(c, s, seq, n_pairs, k0_fmt) != VDL2GPU_OK) { c->use_graphs = false; graph = false; }
 	vdl2_k1_params p1; vdl2_k2a_params pa; vdl2_k2_params p2; vdl2_k3_params p3;
 	fill_params(c, s, seq, n_pairs, c->decim_cnt, s.n_dec, c->last_n_dec, s.dec_base, nullptr, p1, pa, p2, p3);
+	if(c->d_spec) fill_spectrum(c, s, n_pairs);
 	if(graph) {
 		s.h_args->raw = d_raw; s.h_args->dec_base = s.dec_base; s.h_args->n_pairs = n_pairs; s.h_args->cnt0 = c->decim_cnt;
 		s.h_args->n_dec = s.n_dec; s.h_args->prev_n_dec = c->last_n_dec;
@@ -1067,6 +1116,13 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 		KL(vdl2_launch_k1(&p1, (c->cfg.flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->stream));
 	}
 	if(s.timed) CU(cudaEventRecord(s.tk[2], c->stream));
+	if(c->d_spec && !graph) {
+		/* a restart span (never captured) zeroes its restarting receivers' figures first */
+		for(uint32_t r : c->spec_zero) CU(cudaMemsetAsync(c->d_spec + r, 0, sizeof(vdl2_spec_acc), c->stream));
+		c->spec_zero.clear();
+		int rc = launch_spectrum(c, s, n_pairs);
+		if(rc) return rc;
+	}
 	CU(cudaEventRecord(c->ev_input_consumed, c->stream));
 	CU(cudaEventRecord(c->ev_k1_done[db], c->stream));
 	/* ---- middle stage: K2a -> plane[pb] (free once K2 of chunk c-2 is done), history from plane[pb ^ 1] (chunk c-1, same stream) ---- */
@@ -1251,6 +1307,7 @@ static void fill_restarts(vdl2gpu_ctx *c, chunk_slot &s) {
 			e.dphi = vdl2_nco_dphi(c->rx_centre[r], c->freqs[chan], rate);
 			e.freq = c->freqs[chan];
 		}
+		if(c->d_spec) { c->spec_pos[r] = 0; c->spec_zero.push_back(r); }    /* a new segment grid from this span on */
 		c->rx_restart_pending[r] = 0;
 	}
 	c->n_restart_pending = 0;
@@ -1628,6 +1685,13 @@ static int migrate_receivers(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const vdl2gpu_recei
 		for(uint32_t r = 0; r < n_rx; r++) if(from[r] >= 0) new_lv[r] = old_lv[from[r]];
 		CU(cudaMemcpyAsync(n->d_levels, new_lv.data(), new_lv.size() * sizeof(vdl2_levels), cudaMemcpyHostToDevice, c->stream));
 	}
+	/* spectrum: likewise, with its waiting samples and its place on its segment grid */
+	if(c->d_spec)
+		for(uint32_t r = 0; r < n_rx; r++) {
+			if(from[r] < 0) continue;
+			CU(cudaMemcpyAsync(n->d_spec + r, c->d_spec + from[r], sizeof(vdl2_spec_acc), cudaMemcpyDeviceToDevice, c->stream));
+			n->spec_pos[r] = c->spec_pos[from[r]];
+		}
 	CU(cudaStreamSynchronize(c->stream));
 	/* per receiver: a kept one carries its position and a pending restart over; every history now starts at row 0 */
 	for(uint32_t r = 0; r < n_rx; r++) {
@@ -1867,6 +1931,34 @@ extern "C" int vdl2gpu_get_input_levels(vdl2gpu_ctx *c, vdl2gpu_input_levels *ou
 		o.clipped = lv[k].clipped;
 		o.peak = lv[k].peak;
 		o.full_scale = vdl2_level_full_scale(c->mixed ? c->rx_in[k].fmt : c->cfg.sample_fmt);
+	}
+	return VDL2GPU_OK;
+}
+
+/* Spectrum (VDL2GPU_FLAG_SPECTRUM): out[k] for inputs [first, first + n), after everything submitted so far has run */
+extern "C" int vdl2gpu_get_spectrum(vdl2gpu_ctx *c, uint32_t first, uint32_t n, vdl2gpu_spectrum *out) {
+	const char *why = nullptr;
+	if(!c) why = "no context";
+	else if(!out) why = "no output";
+	else if(!c->d_spec) why = "the context was created without VDL2GPU_FLAG_SPECTRUM";
+	else if((uint64_t)first + n > c->n_streams) why = "inputs asked for past the context's last input";
+	if(why) {
+		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_get_spectrum: %s", why);
+		return VDL2GPU_EINVAL;
+	}
+	if(n == 0) return VDL2GPU_OK;
+	CU(cudaSetDevice(c->device));
+	CU(cudaStreamSynchronize(c->stream));
+	CU(cudaStreamSynchronize(c->s_back));
+	const vdl2_spec_acc *a = c->d_spec + first;
+	CU(cudaMemcpy2D(out->pow_lo, sizeof(vdl2gpu_spectrum), a->lo, sizeof(vdl2_spec_acc), sizeof(a->lo), n, cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy2D(out->pow_hi, sizeof(vdl2gpu_spectrum), a->hi, sizeof(vdl2_spec_acc), sizeof(a->hi), n, cudaMemcpyDeviceToHost));
+	CU(cudaMemcpy2D(out->peak, sizeof(vdl2gpu_spectrum), a->peak, sizeof(vdl2_spec_acc), sizeof(a->peak), n, cudaMemcpyDeviceToHost));
+	for(uint32_t k = 0; k < n; k++) {
+		const uint64_t pos = c->spec_pos[first + k];
+		out[k].segments = pos >> VDL2_SPEC_LOG2N;
+		out[k].pending = (uint32_t)(pos & (VDL2_SPEC_N - 1u));
+		out[k].reserved = 0;
 	}
 	return VDL2GPU_OK;
 }

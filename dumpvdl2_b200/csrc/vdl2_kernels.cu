@@ -1683,6 +1683,9 @@ template<typename K> static void vdl2_set_carveout(K kernel, int pct) {
 	if(pct >= 0) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
 }
 
+__global__ void k_spectrum(const float2 *__restrict__ samples, uint32_t stride, uint32_t lanes, uint32_t full_warps,
+		const vdl2_spec_span *__restrict__ span, const vdl2_spec_tab *__restrict__ tab, vdl2_spec_acc *__restrict__ acc);
+
 static std::once_flag g_dev_once[64];
 
 extern "C" int vdl2_kernels_init_device(int device) {
@@ -1756,6 +1759,7 @@ extern "C" int vdl2_kernels_init_device(int device) {
 		vdl2_set_carveout(k3_burst_fec, pct);
 		vdl2_set_carveout(k3_burst_fec_abandoned, pct);
 		vdl2_set_carveout(k_chunk_finish, pct);
+		vdl2_set_carveout(k_spectrum, pct);
 	});
 	return (int)cudaGetLastError();
 }
@@ -2003,5 +2007,120 @@ __global__ void __launch_bounds__(256) k_migrate_receivers(vdl2_migrate_params p
 extern "C" int vdl2_launch_migrate(const vdl2_migrate_params *p, cudaStream_t st) {
 	if(p->chlv) k_migrate_receivers<true><<<(p->n_chp + 255u) / 256u, 256, 0, st>>>(*p);
 	else k_migrate_receivers<false><<<(p->n_chp + 255u) / 256u, 256, 0, st>>>(*p);
+	return (int)cudaGetLastError();
+}
+
+/* ------------------------------------------------------------------------------------------------
+ * Spectrum (VDL2GPU_FLAG_SPECTRUM): block (i, g) takes input i's segments [g SPEC_SPB, (g + 1) SPEC_SPB) of the chunk, one
+ * at a time, through the butterflies of vdl2_core.cuh in shared memory, and keeps the sums and peaks of its four bins per
+ * thread in registers; it adds them to the input's accumulators once, with the carry rule of vdl2_pow_carry, so the totals
+ * are exact in any block order.  Block (i, 0) then keeps the samples of the input's incomplete segment: it alone reads
+ * the carry (only segment 0 starts in it), and it writes the carry only after that.
+ *   - Two stages per pass: a thread takes the four elements that stages s and s + 1 combine among themselves into
+ *     registers and runs the same four butterflies the serial vdl2_spec_segment runs on them, so 5 passes and barriers
+ *     instead of 10.  Every butterfly keeps its inputs and twiddle: the result is bit for bit the host's.
+ *   - Shared memory is padded by one element per 32 (spec_at), so the bit-reversed stores of a warp, which are 32
+ *     elements apart, fall into different banks.
+ *   - The next segment's samples are loaded into registers before the current segment's butterflies.
+ * The grid runs inputs along x, so that in the one-stream-per-channel layout the blocks of neighbouring columns run
+ * together and share the 32-byte sectors of each row through L2.
+ * ---------------------------------------------------------------------------------------------- */
+#define SPEC_THREADS 256u
+#define SPEC_SPB 16u        /* segments per block: one set of atomics per bin for 16 segments */
+#define SPEC_PER_THREAD (VDL2_SPEC_N / SPEC_THREADS)
+
+__device__ __forceinline__ uint32_t spec_at(uint32_t n) { return n + (n >> 5); }
+
+__global__ void __launch_bounds__(SPEC_THREADS, 3) k_spectrum(const float2 *__restrict__ samples, uint32_t stride, uint32_t lanes, uint32_t full_warps,
+		const vdl2_spec_span *__restrict__ span, const vdl2_spec_tab *__restrict__ tab, vdl2_spec_acc *__restrict__ acc) {
+	__shared__ float2 buf[VDL2_SPEC_N + VDL2_SPEC_N / 32];
+	__shared__ float2 tw[VDL2_SPEC_N / 2];
+	const uint32_t i = blockIdx.x, g = blockIdx.y, tid = threadIdx.x;
+	const vdl2_spec_span e = span[i];
+	const uint32_t nseg = vdl2_spec_segments(e);
+	const uint32_t j0 = g * SPEC_SPB, j1 = min(j0 + SPEC_SPB, nseg);
+	if(j0 >= j1 && g != 0) return;                          /* (uniform over the block) */
+	const size_t base = lanes ? (size_t)vdl2_channel_slot(i, lanes, full_warps) : (size_t)i * stride;
+	const size_t step = lanes ? stride : 1u;
+	vdl2_spec_acc &a = acc[i];
+	float w[SPEC_PER_THREAD];
+	uint64_t lo[SPEC_PER_THREAD], hi[SPEC_PER_THREAD];
+	uint32_t pk[SPEC_PER_THREAD];
+	float2 x[SPEC_PER_THREAD];
+#pragma unroll
+	for(uint32_t m = 0; m < SPEC_PER_THREAD; m++) { w[m] = tab->win[tid + m * SPEC_THREADS]; lo[m] = hi[m] = 0; pk[m] = 0; }
+	for(uint32_t k = tid; k < VDL2_SPEC_N / 2; k += SPEC_THREADS) tw[k] = tab->tw[k];
+	auto load = [&](uint32_t j) {
+#pragma unroll
+		for(uint32_t m = 0; m < SPEC_PER_THREAD; m++) {
+			const int64_t t = vdl2_spec_src(e, j, tid + m * SPEC_THREADS);
+			x[m] = t >= 0 ? samples[base + (size_t)t * step] : a.carry[e.pend + t];
+		}
+	};
+	if(j0 < j1) load(j0);
+	for(uint32_t j = j0; j < j1; j++) {
+		__syncthreads();                                      /* the twiddles are in; the previous segment's bins are read */
+#pragma unroll
+		for(uint32_t m = 0; m < SPEC_PER_THREAD; m++) {
+			const uint32_t n = tid + m * SPEC_THREADS;
+			buf[spec_at(vdl2_spec_bitrev(n))] = vdl2_spec_windowed(x[m], w[m]);
+		}
+		if(j + 1 < j1) load(j + 1);
+#pragma unroll
+		for(uint32_t s = 0; s < VDL2_SPEC_LOG2N; s += 2) {
+			__syncthreads();
+			/* stages s and s + 1 (h = 2^s): the thread's elements are q + {0, h, 2h, 3h}, q = (tid / h) 4h + tid mod h;
+			 * stage s pairs (0, h) and (2h, 3h), which are butterflies b and b + h of it, stage s + 1 pairs (0, 2h) and
+			 * (h, 3h), butterflies b and b + h of that stage, with b = (tid / h) 2h + tid mod h */
+			const uint32_t h = 1u << s, b = ((tid >> s) << (s + 1)) + (tid & (h - 1u));
+			uint32_t q, q1, k0, k1, k2, k3;
+			vdl2_spec_pair(s, b, q, q1, k0);
+			vdl2_spec_pair(s, b + h, q1, q1, k1);
+			vdl2_spec_pair(s + 1u, b, q1, q1, k2);
+			vdl2_spec_pair(s + 1u, b + h, q1, q1, k3);
+			float2 v0 = buf[spec_at(q)], v1 = buf[spec_at(q + h)], v2 = buf[spec_at(q + 2u * h)], v3 = buf[spec_at(q + 3u * h)];
+			vdl2_spec_bfly(v0, v1, tw[k0]);
+			vdl2_spec_bfly(v2, v3, tw[k1]);
+			vdl2_spec_bfly(v0, v2, tw[k2]);
+			vdl2_spec_bfly(v1, v3, tw[k3]);
+			buf[spec_at(q)] = v0; buf[spec_at(q + h)] = v1; buf[spec_at(q + 2u * h)] = v2; buf[spec_at(q + 3u * h)] = v3;
+		}
+		__syncthreads();
+#pragma unroll
+		for(uint32_t m = 0; m < SPEC_PER_THREAD; m++) {
+			const float2 v = buf[spec_at(vdl2_spec_fft_bin(tid + m * SPEC_THREADS))];
+			const float p = vdl2_chlv_pow(v.x, v.y);
+			vdl2_pow_fold(lo[m], hi[m], vdl2_spec_q(p));
+			pk[m] = max(pk[m], vdl2_f32_bits(p));
+		}
+	}
+	if(j1 > j0) {
+#pragma unroll
+		for(uint32_t m = 0; m < SPEC_PER_THREAD; m++) {
+			const uint32_t k = tid + m * SPEC_THREADS;
+			if(lo[m] | hi[m]) {
+				const uint64_t old = atomicAdd(reinterpret_cast<unsigned long long *>(&a.lo[k]), (unsigned long long)lo[m]);
+				const uint64_t h = hi[m] + vdl2_pow_carry(old, lo[m]);
+				if(h) atomicAdd(reinterpret_cast<unsigned long long *>(&a.hi[k]), (unsigned long long)h);
+			}
+			if(pk[m]) atomicMax(&a.peak[k], pk[m]);
+		}
+	}
+	if(g == 0) {
+		__syncthreads();                                      /* segment 0 has read the carry */
+		const uint32_t rest = vdl2_spec_rest(e);
+		for(uint32_t k = tid; k < rest; k += SPEC_THREADS) {
+			const int64_t t = vdl2_spec_src(e, nseg, k);
+			if(t >= 0) a.carry[k] = samples[base + (size_t)t * step];    /* (t < 0: a sample already held, in its place) */
+		}
+	}
+}
+
+extern "C" int vdl2_launch_spectrum(const float *samples, uint32_t width, uint32_t n_in, uint32_t stride, uint32_t lanes, uint32_t full_warps,
+		const vdl2_spec_span *span, const vdl2_spec_tab *tab, vdl2_spec_acc *acc, cudaStream_t st) {
+	if(width == 0 || n_in == 0) return 0;
+	const uint32_t most_segs = (uint32_t)(((uint64_t)width + VDL2_SPEC_N - 1u) / VDL2_SPEC_N);   /* with up to N - 1 held */
+	k_spectrum<<<dim3(n_in, (most_segs + SPEC_SPB - 1u) / SPEC_SPB), SPEC_THREADS, 0, st>>>(reinterpret_cast<const float2 *>(samples), stride,
+			lanes, full_warps, span, tab, acc);
 	return (int)cudaGetLastError();
 }

@@ -188,6 +188,12 @@ int vdl2_launch_k3(const vdl2_k3_params *p, uint32_t grid, cudaStream_t st);
 int vdl2_launch_k4(const uint8_t *frames, const uint32_t *offsets, const uint32_t *lens, uint32_t n, uint16_t *out, cudaStream_t st);
 int vdl2_launch_rs(uint8_t *blocks, const int32_t *fec_octets, uint32_t n, int32_t *ret, const vdl2_tables *tables, cudaStream_t st);
 int vdl2_launch_migrate(const vdl2_migrate_params *p, cudaStream_t st);
+/* Spectrum (VDL2GPU_FLAG_SPECTRUM): n_in inputs of the sample plane, input i bringing span[i].n samples after span[i].pend
+ * held in acc[i].carry (vdl2_core.cuh).  Input i's sample t is samples[i x stride + t] (row layouts), or, with lanes != 0
+ * (one stream per channel, time-major), samples[t x stride + slot of i].  width: the most samples any input brings (sizes
+ * the grid). */
+int vdl2_launch_spectrum(const float *samples, uint32_t width, uint32_t n_in, uint32_t stride, uint32_t lanes, uint32_t full_warps,
+		const vdl2_spec_span *span, const vdl2_spec_tab *tab, vdl2_spec_acc *acc, cudaStream_t st);
 #ifdef __cplusplus
 }
 #endif

@@ -55,8 +55,10 @@ enum {
 	VDL2GPU_FLAG_RAGGED = 1u << 5,       /* vdl2gpu_create_mixed_receivers only: every receiver brings its own number of decimated
 	                                      * samples to a span (vdl2gpu_submit_ragged); every other create function refuses it */
 	VDL2GPU_FLAG_INPUT_LEVELS = 1u << 6, /* measure every input's levels on the device (vdl2gpu_get_input_levels); any create function */
-	VDL2GPU_FLAG_CHANNEL_LEVELS = 1u << 7 /* measure every channel's in-band levels on the device (vdl2gpu_get_channel_levels); any
+	VDL2GPU_FLAG_CHANNEL_LEVELS = 1u << 7, /* measure every channel's in-band levels on the device (vdl2gpu_get_channel_levels); any
 	                                       * create function */
+	VDL2GPU_FLAG_SPECTRUM = 1u << 8      /* measure every input's power spectrum on the device (vdl2gpu_get_spectrum); any create
+	                                      * function */
 };
 
 typedef struct {
@@ -389,6 +391,45 @@ typedef struct {
  * or output, n larger than the number of channels, or a context created without VDL2GPU_FLAG_CHANNEL_LEVELS.  Not
  * available through the stage stubs or the drop-in symbols. */
 int vdl2gpu_get_channel_levels(vdl2gpu_ctx *ctx, vdl2gpu_channel_levels *out, uint32_t n);
+
+/* Spectrum (VDL2GPU_FLAG_SPECTRUM): the power spectrum of every input in VDL2GPU_SPECTRUM_BINS bins, for seeing what lies
+ * between and beside the configured channels: an interferer, a DC spike, a receiver tuned off, traffic on a slot not yet
+ * configured, a filter edge.  Inputs are numbered as for vdl2gpu_get_input_levels.
+ *   - Segment j of an input is its complex samples [1024 j, 1024 (j + 1)), counted from create (for a receiver added by
+ *     vdl2gpu_update_receivers: from when it joined; after vdl2gpu_restart_receiver: from the restart).  A segment counts
+ *     once its last sample has been in a chunk or span that ran; the samples of the segment not yet complete (at most 1023)
+ *     wait on the device.
+ *   - Per segment, with x_n the float the reference makes of sample n (cu8 c / 255, cs16 v / 32768): y_n = fl32(x_n w_n),
+ *     w the periodic Hann window 0.5 - 0.5 cos(2 pi n / 1024) rounded to float; a radix-2 FFT with float twiddles, every
+ *     product and sum rounded on its own; p_k = fl32(fl32(re^2) + fl32(im^2)).  Bin k (stored order) is the frequency
+ *     centre + (k - 512) fs / 1024, fs = 105000 x the input's oversample: bin 512 is the centre.
+ *   - pow[k] = pow_hi[k] x 2^64 + pow_lo[k] is the exact sum over segments of (uint64)(p_k x 2^40); peak[k] the largest p_k
+ *     (peak hold).  A full-scale complex tone on a bin gives p = 512^2, so the mean power in dBFS is
+ *     10 log10(pow / 2^40 / segments / 512^2).
+ *   - The figures do not depend on how the stream was cut (chunk, span and push lengths, ragged counts), n_inflight, graphs,
+ *     trace or VDL2GPU_FLAG_NO_OVERLAP.  Pushed input counts once it enters a span; bytes still queued, or dropped by a
+ *     restart, never count.
+ *   - vdl2gpu_restart_receiver zeroes the receiver's spectrum and drops its waiting samples at the span the restart applies
+ *     to: a retune changes what every bin means.  Read the old figures first (this call waits for everything submitted).
+ *     vdl2gpu_update_receivers: a kept receiver carries its figures and waiting samples to its new index, a new receiver
+ *     starts at zero, a removed receiver's figures are gone.
+ *   - Frames, metadata, counters, trace events, vdl2gpu_stats and both levels are the same with the flag on or off.  A
+ *     context without the flag allocates and launches nothing for it.  With it, a context holds 28 KB of device memory per
+ *     input (the sums, the peaks and the waiting samples), about 460 MB at 16384 one-channel receivers. */
+#define VDL2GPU_SPECTRUM_BINS 1024
+typedef struct {
+	uint64_t segments;                              /* complete segments counted */
+	uint32_t pending;                               /* samples of the incomplete segment held on the device, 0..1023 */
+	uint32_t reserved;
+	uint64_t pow_lo[VDL2GPU_SPECTRUM_BINS];         /* sum of (uint64)(p_k 2^40), one unsigned 128-bit integer per bin */
+	uint64_t pow_hi[VDL2GPU_SPECTRUM_BINS];
+	float peak[VDL2GPU_SPECTRUM_BINS];              /* largest p_k */
+} vdl2gpu_spectrum;                                 /* 20496 bytes */
+/* out[k] = the spectrum of input first + k for k < n, after everything submitted so far has run.  Runs on the control
+ * thread, concurrently with vdl2gpu_push.  VDL2GPU_EINVAL (with vdl2gpu_last_error) for a NULL context or output, a range
+ * past the inputs, or a context created without VDL2GPU_FLAG_SPECTRUM.  Not available through the stage stubs or the
+ * drop-in symbols. */
+int vdl2gpu_get_spectrum(vdl2gpu_ctx *ctx, uint32_t first, uint32_t n, vdl2gpu_spectrum *out);
 
 /* ---- multi-GPU ingest (one process per GPU; global channel k is demodulated on GPU k mod N, the reference's
  * channel threads share nothing but the read-only sample buffer: src/dumpvdl2.c:117-135, src/demod.c:50,300-301).
