@@ -147,7 +147,6 @@ struct vdl2gpu_ctx {
 	uint32_t k2a_split = 64;                            /* time slices of the K2a grid (VDL2GPU_K2A_SPLIT) */
 	int stages = 2;                                     /* 2: K2a runs alone between K1 of chunk c and K1 of chunk c+1 (default, see run_chain);
 	                                                     * 3: K2a of chunk c+1 beside K1 of chunk c+2 and K2 of chunk c (VDL2GPU_STAGES=3) */
-	bool k2a_exclusive = true;                          /* K1 of chunk c+1 waits for K2a of chunk c (VDL2GPU_K2A_EXCLUSIVE=0: let them overlap) */
 	uint64_t overflows_reported = 0;
 	host_tables tab;
 	vdl2_tables *d_tab = nullptr;
@@ -563,7 +562,6 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 		if((e = getenv("VDL2GPU_K2A"))) c->k2a_mode = atoi(e);
 		if((e = getenv("VDL2GPU_NO_GRAPH")) && atoi(e)) c->use_graphs = false;
 		if((e = getenv("VDL2GPU_BLOCK_TRACE")) && atoi(e)) c->block_trace_cap = 1u << 16;
-		if((e = getenv("VDL2GPU_K2A_EXCLUSIVE"))) c->k2a_exclusive = atoi(e) != 0;
 		if((e = getenv("VDL2GPU_STAGES")) && atoi(e) == 3) { c->stages = 3; c->k2a_split = 3; }
 		if((e = getenv("VDL2GPU_K2A_SPLIT")) && atoi(e) >= 1 && atoi(e) <= 256) c->k2a_split = (uint32_t)atoi(e);
 	}
@@ -958,10 +956,11 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
  * (n_pairs) and replayed: a chunk then costs three graph launches and a handful of event calls instead of seven kernel
  * launches.  Everything that differs between two chunks of the same shape (input pointer, decimation phase, sample
  * counts, absolute sample index) travels in the chunk-argument block the front graph copies to the device first. */
-static int capture_one(cudaStream_t st, cudaGraphExec_t *out, int (*body)(void *), void *arg) {
+template<typename F>
+static int capture_one(cudaStream_t st, cudaGraphExec_t *out, F body) {
 	cudaGraph_t g = nullptr;
 	CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed));
-	int rc = body(arg);
+	int rc = body();
 	cudaError_t e = cudaStreamEndCapture(st, &g);
 	if(rc != 0 || e != cudaSuccess) { if(g) cudaGraphDestroy(g); cudaGetLastError(); return rc ? rc : fail_cuda(e, "cudaStreamEndCapture", __LINE__); }
 	e = cudaGraphInstantiate(out, g, 0);
@@ -973,23 +972,18 @@ static int capture_one(cudaStream_t st, cudaGraphExec_t *out, int (*body)(void *
 /* input samples per decimated sample as the chain counts them: a mixed-rate context counts decimated samples directly */
 static inline uint32_t chain_os(const vdl2gpu_ctx *c) { return c->mixed ? 1u : c->cfg.oversample; }
 
-/* mixed-rate receivers: K0 of a span of n_dec decimated samples into the sample plane (ca: graph replay) */
-static int launch_k0_mixed(vdl2gpu_ctx *c, const void *d_raw, uint32_t n_dec, const vdl2_chunk_args *ca) {
-	KL(vdl2_launch_k0_mixed(d_raw, n_dec, c->d_rx_in, c->n_streams, c->rx_os_max, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples),
-			c->max_pairs, ca, c->d_levels, c->stream));
-	return VDL2GPU_OK;
-}
-
-/* mixed-rate receivers: K0 of a span of n_dec decimated samples (ragged spans: n_dec is the width, the slot's table the counts) */
-static int launch_k0_span(vdl2gpu_ctx *c, const chunk_slot &s, const void *d_raw, uint32_t n_dec, const vdl2_chunk_args *ca) {
-	if(!c->ragged) return launch_k0_mixed(c, d_raw, n_dec, ca);
-	if(s.pushed) {                                      /* (never captured: pushed spans take the direct path) */
-		KL(vdl2_launch_k0_rings(c->d_rings, n_dec, c->d_rx_in, c->d_ring_tab, s.d_span, c->n_streams, c->rx_os_max, c->d_tab->levels,
-				reinterpret_cast<float *>(c->d_samples), c->max_pairs, c->d_levels, c->stream));
-		return VDL2GPU_OK;
-	}
-	KL(vdl2_launch_k0_ragged(d_raw, n_dec, c->d_rx_in, s.d_span, c->n_streams, c->rx_os_max, c->d_tab->levels,
-			reinterpret_cast<float *>(c->d_samples), c->max_pairs, ca, c->d_levels, c->stream));
+/* K0 of a chunk into the sample plane: one row per receiver (mixed-rate receivers; ragged spans, whose table gives the
+ * counts, and pushed spans, which read the receivers' rings), one column per stream (one stream per channel) or one row
+ * per stream.  n_pairs: samples per stream, or the span's decimated samples (its width when ragged).  ca: graph capture. */
+static int launch_k0(vdl2gpu_ctx *c, const chunk_slot &s, const void *raw, uint32_t n_pairs, uint32_t fmt, const vdl2_chunk_args *ca) {
+	float *out = reinterpret_cast<float *>(c->d_samples);
+	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
+	if(c->mixed) {
+		const vdl2_k0_rows rows = { s.pushed ? c->d_rings : raw, c->d_rx_in, s.d_span, s.pushed ? c->d_ring_tab : nullptr };
+		KL(vdl2_launch_k0_rows(&rows, n_pairs, c->n_streams, c->rx_os_max, c->d_tab->levels, out, c->max_pairs, ca, c->d_levels, c->stream));
+	} else if(c->lane_streams) KL(vdl2_launch_k0_lanes(raw, n_pairs, fmt, c->d_tab->levels, out, c->n_streams, n_pairs * bpp, c->n_chp,
+			c->lanes, c->full_warps, ca, c->d_levels, c->stream));
+	else KL(vdl2_launch_k0(raw, n_pairs, fmt, c->d_tab->levels, out, c->n_streams, n_pairs * bpp, c->max_pairs, ca, c->d_levels, c->stream));
 	return VDL2GPU_OK;
 }
 
@@ -1012,41 +1006,41 @@ static void fill_spectrum(vdl2gpu_ctx *c, chunk_slot &s, uint32_t n_pairs) {
 	}
 }
 
-struct capture_env { vdl2gpu_ctx *c; chunk_slot *s; uint64_t seq; uint32_t n_pairs; uint32_t k0_fmt; };
-#define CAPTURE_PARAMS \
-	capture_env *e = static_cast<capture_env *>(a); \
-	vdl2gpu_ctx *c = e->c; \
-	vdl2_k1_params p1; vdl2_k2a_params pa; vdl2_k2_params p2; vdl2_k3_params p3; \
-	const uint32_t os = chain_os(c); \
-	fill_params(c, *e->s, e->seq, e->n_pairs, 0, (os - 1 + e->n_pairs) / os, 0, 0, e->s->d_args, p1, pa, p2, p3)
-
-static int body_front(void *a) {
-	CAPTURE_PARAMS;
-	(void)pa; (void)p2; (void)p3;
-	CU(cudaMemcpyAsync(e->s->d_args, e->s->h_args, sizeof(vdl2_chunk_args), cudaMemcpyHostToDevice, c->stream));
-	if(c->ragged) CU(cudaMemcpyAsync(e->s->d_span, e->s->h_span, c->n_streams * sizeof(vdl2_rx_span), cudaMemcpyHostToDevice, c->stream));
-	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
-	if(c->mixed) { int rc = launch_k0_span(c, *e->s, nullptr, e->n_pairs, e->s->d_args); if(rc) return rc; }
-	else if(c->lane_streams) KL(vdl2_launch_k0_lanes(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-			e->n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, e->s->d_args, c->d_levels, c->stream));
-	else KL(vdl2_launch_k0(nullptr, e->n_pairs, e->k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-			e->n_pairs * bpp, c->max_pairs, e->s->d_args, c->d_levels, c->stream));
+/* Front stage of a chunk on the front stream: K0, K1 and the spectrum.  ca: captured into the front graph (the chunk's
+ * values then come from the device copy of its arguments), NULL on the direct path. */
+static int launch_front(vdl2gpu_ctx *c, chunk_slot &s, const void *raw, uint32_t n_pairs, uint32_t k0_fmt, const vdl2_k1_params &p1,
+		const vdl2_chunk_args *ca) {
+	/* only a replay needs the chunk's arguments on the device */
+	if(ca) CU(cudaMemcpyAsync(s.d_args, s.h_args, sizeof(vdl2_chunk_args), cudaMemcpyHostToDevice, c->stream));
+	if(c->ragged) CU(cudaMemcpyAsync(s.d_span, s.h_span, c->n_streams * sizeof(vdl2_rx_span), cudaMemcpyHostToDevice, c->stream));
+	/* restart spans and pushed spans are never captured */
+	if(!ca && s.restart) CU(cudaMemcpyAsync(s.d_restart, s.h_restart, c->n_chp * sizeof(vdl2_rx_restart), cudaMemcpyHostToDevice, c->stream));
+	int rc = launch_k0(c, s, raw, n_pairs, k0_fmt, ca);
+	if(rc) return rc;
+	if(!ca && s.pushed) CU(cudaEventRecord(s.k0_done, c->stream));     /* the rings' bytes of this span are read */
+	/* the direct path times K0 and K1 apart; a replayed front graph is timed as a whole (run_chain) */
+	const bool timed = !ca && s.timed;
+	if(timed) CU(cudaEventRecord(s.tk[1], c->stream));
 	KL(vdl2_launch_k1(&p1, (c->cfg.flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->stream));
-	if(c->d_spec) { int rc = launch_spectrum(c, *e->s, e->n_pairs); if(rc) return rc; }
-	return 0;
+	if(timed) CU(cudaEventRecord(s.tk[2], c->stream));
+	if(c->d_spec) {
+		if(!ca) {       /* a restart span (never captured) zeroes its restarting receivers' figures first */
+			for(uint32_t r : c->spec_zero) CU(cudaMemsetAsync(c->d_spec + r, 0, sizeof(vdl2_spec_acc), c->stream));
+			c->spec_zero.clear();
+		}
+		rc = launch_spectrum(c, s, n_pairs);
+		if(rc) return rc;
+	}
+	return VDL2GPU_OK;
 }
-static int body_k2a(void *a) {
-	CAPTURE_PARAMS;
-	(void)p1; (void)p2; (void)p3;
-	KL(vdl2_launch_k2a_warps(&pa, c->s_mid));
-	return 0;
-}
-static int body_back(void *a) {
-	CAPTURE_PARAMS;
-	(void)p1; (void)pa;
+
+/* Back stage of a chunk on the back stream: K2, K3.  tk_k2 (or NULL) is recorded between them: the direct path times them
+ * apart, a replayed back graph as a whole. */
+static int launch_back(vdl2gpu_ctx *c, const vdl2_k2_params &p2, const vdl2_k3_params &p3, cudaEvent_t tk_k2) {
 	KL(vdl2_launch_k2(&p2, c->s_back));
+	if(tk_k2) CU(cudaEventRecord(tk_k2, c->s_back));
 	KL(vdl2_launch_k3(&p3, K3_GRID, c->s_back));
-	return 0;
+	return VDL2GPU_OK;
 }
 
 static int ensure_graphs(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_pairs, uint32_t k0_fmt) {
@@ -1055,10 +1049,12 @@ static int ensure_graphs(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n
 	if(s.g_front[k]) { cudaGraphExecDestroy(s.g_front[k]); s.g_front[k] = nullptr; }
 	if(s.g_k2a[k]) { cudaGraphExecDestroy(s.g_k2a[k]); s.g_k2a[k] = nullptr; }
 	if(s.g_back[k]) { cudaGraphExecDestroy(s.g_back[k]); s.g_back[k] = nullptr; }
-	capture_env e = { c, &s, seq, n_pairs, k0_fmt };
-	int rc = capture_one(c->stream, &s.g_front[k], body_front, &e);
-	if(rc == 0) rc = capture_one(c->s_mid, &s.g_k2a[k], body_k2a, &e);
-	if(rc == 0) rc = capture_one(c->s_back, &s.g_back[k], body_back, &e);
+	vdl2_k1_params p1; vdl2_k2a_params pa; vdl2_k2_params p2; vdl2_k3_params p3;
+	const uint32_t os = chain_os(c);
+	fill_params(c, s, seq, n_pairs, 0, (os - 1 + n_pairs) / os, 0, 0, s.d_args, p1, pa, p2, p3);
+	int rc = capture_one(c->stream, &s.g_front[k], [&] { return launch_front(c, s, nullptr, n_pairs, k0_fmt, p1, s.d_args); });
+	if(rc == 0) rc = capture_one(c->s_mid, &s.g_k2a[k], [&] { KL(vdl2_launch_k2a_warps(&pa, c->s_mid)); return 0; });
+	if(rc == 0) rc = capture_one(c->s_back, &s.g_back[k], [&] { return launch_back(c, p2, p3, nullptr); });
 	if(rc == 0) s.graph_pairs[k] = n_pairs;
 	return rc;
 }
@@ -1076,7 +1072,6 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	s.timed = c->timing;
 	const uint64_t seq = c->chunk_seq;
 	const int db = (int)(seq % 3u), pb = (int)(seq & 1u), gk = (int)(seq % 6u);
-	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
 	const bool overlap = c->s_back != c->stream;
 	s.seq = seq;
 	bool graph = c->use_graphs && !planar && overlap && !s.pushed;     /* pushed spans take the direct path */
@@ -1098,29 +1093,14 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 	 * empty machine together, one block per SM each - the only arrangement in which the block scheduler was found to keep
 	 * the two long kernels side by side on every SM, launch after launch (see the slot mapping in create_impl). */
 	if(c->stages == 2 && seq >= 1 && overlap) CU(cudaStreamWaitEvent(c->stream, c->ev_k2a_done[pb ^ 1], 0));
-	if(s.timed) { CU(cudaEventRecord(s.tk[0], c->stream)); if(graph) CU(cudaEventRecord(s.tk[1], c->stream)); }
+	if(s.timed) CU(cudaEventRecord(s.tk[0], c->stream));
 	if(graph) {
-		CU(cudaGraphLaunch(s.g_front[gk], c->stream));
-	} else {
-		if(c->ragged) CU(cudaMemcpyAsync(s.d_span, s.h_span, c->n_streams * sizeof(vdl2_rx_span), cudaMemcpyHostToDevice, c->stream));
-		if(s.restart) CU(cudaMemcpyAsync(s.d_restart, s.h_restart, c->n_chp * sizeof(vdl2_rx_restart), cudaMemcpyHostToDevice, c->stream));
-		if(c->mixed) {
-			int rc = launch_k0_span(c, s, d_raw, n_pairs, nullptr);
-			if(rc) return rc;
-			if(s.pushed) CU(cudaEventRecord(s.k0_done, c->stream));     /* the rings' bytes of this span are read */
-		} else if(c->lane_streams) KL(vdl2_launch_k0_lanes(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-				n_pairs * bpp, c->n_chp, c->lanes, c->full_warps, nullptr, c->d_levels, c->stream));
-		else KL(vdl2_launch_k0(d_raw, n_pairs, k0_fmt, c->d_tab->levels, reinterpret_cast<float *>(c->d_samples), c->n_streams,
-				n_pairs * bpp, c->max_pairs, nullptr, c->d_levels, c->stream));
+		/* timed as a whole: the spectrum falls inside "K1" */
 		if(s.timed) CU(cudaEventRecord(s.tk[1], c->stream));
-		KL(vdl2_launch_k1(&p1, (c->cfg.flags & VDL2GPU_FLAG_K1_SCALAR) ? 1 : 0, c->k1_variant, c->stream));
-	}
-	if(s.timed) CU(cudaEventRecord(s.tk[2], c->stream));
-	if(c->d_spec && !graph) {
-		/* a restart span (never captured) zeroes its restarting receivers' figures first */
-		for(uint32_t r : c->spec_zero) CU(cudaMemsetAsync(c->d_spec + r, 0, sizeof(vdl2_spec_acc), c->stream));
-		c->spec_zero.clear();
-		int rc = launch_spectrum(c, s, n_pairs);
+		CU(cudaGraphLaunch(s.g_front[gk], c->stream));
+		if(s.timed) CU(cudaEventRecord(s.tk[2], c->stream));
+	} else {
+		int rc = launch_front(c, s, d_raw, n_pairs, k0_fmt, p1, nullptr);
 		if(rc) return rc;
 	}
 	CU(cudaEventRecord(c->ev_input_consumed, c->stream));
@@ -1141,9 +1121,8 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 		if(s.timed) CU(cudaEventRecord(s.tk[4], c->s_back));
 		c->stats.graph_launches += 3;
 	} else {
-		KL(vdl2_launch_k2(&p2, c->s_back));
-		if(s.timed) CU(cudaEventRecord(s.tk[4], c->s_back));
-		KL(vdl2_launch_k3(&p3, K3_GRID, c->s_back));
+		int rc = launch_back(c, p2, p3, s.timed ? s.tk[4] : nullptr);
+		if(rc) return rc;
 	}
 	if(s.timed) CU(cudaEventRecord(s.tk[5], c->s_back));
 	CU(cudaEventRecord(c->ev_back_done[db], c->s_back));

@@ -222,127 +222,117 @@ __global__ void __launch_bounds__(1024) k0_convert_lanes(const uint8_t *__restri
 	}
 }
 
-/* K0 for mixed-rate receivers: grid row r converts receiver r's n_dec x os_r samples, in its own format, from its own
- * place in the span (vdl2_rx_span_offset) into row r of the sample plane; the same arithmetic as k0_convert.  Rows of
- * receivers with a smaller oversample factor than the largest leave their surplus threads idle. */
-__device__ __forceinline__ float2 k0_mixed_sample(const uint8_t *__restrict__ raw, const vdl2_rx_input &in, uint32_t i,
-		const float *__restrict__ levels) {
-	float re, im;
-	if(in.fmt == 0) {                                    /* src/demod.c:343-345, table from :349-354 */
-		uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
-		re = __ldg(&levels[v.x]);
-		im = __ldg(&levels[v.y]);
-	} else {                                             /* src/demod.c:361-363 */
-		/* a cs16 buffer after a cu8 one of odd n_dec x os starts 2 bytes off a 4-byte boundary: two 16-bit loads then */
-		short2 v;
-		if((reinterpret_cast<uintptr_t>(raw) & 3u) == 0) v = reinterpret_cast<const short2 *>(raw)[i];
-		else { const short *s = reinterpret_cast<const short *>(raw) + 2u * i; v = make_short2(s[0], s[1]); }
-		re = __fdiv_rn((float)v.x, 32768.0f);
-		im = __fdiv_rn((float)v.y, 32768.0f);
-	}
-	return make_float2(re, im);
-}
+/* K0 for per-receiver rows (mixed-rate receivers, ragged spans, pushed spans): grid row r converts receiver r's samples,
+ * in its own format, into row r of the sample plane; the same arithmetic as k0_convert.  A row source says how many
+ * samples row r has (count) and where they lie (row: at(i, bpp) is the address of sample i).  Rows shorter than the grid
+ * leave their surplus threads idle. */
 
-/* levels form of k0_mixed_sample: the raw values as well (the same loads and arithmetic) */
-__device__ __forceinline__ float2 k0_mixed_sample_raw(const uint8_t *__restrict__ raw, const vdl2_rx_input &in, uint32_t i,
-		const float *__restrict__ levels, int32_t &vi, int32_t &vq) {
-	if(in.fmt == 0) {
-		uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
+/* a row whose samples follow each other from p on */
+struct k0_run {
+	const uint8_t *p;
+	__device__ const uint8_t *at(uint32_t i, uint32_t bpp) const { return p + (uint64_t)i * bpp; }
+};
+
+/* a row whose samples lie in a ring at p from offset off on, wrapping at cap.  The ring's capacity is a multiple of the
+ * sample size and its tail advances in whole groups, so no sample straddles the wrap and every cs16 sample starts 4-byte
+ * aligned. */
+struct k0_ring_run {
+	const uint8_t *p; uint64_t off, cap;
+	__device__ const uint8_t *at(uint32_t i, uint32_t bpp) const {
+		const uint64_t q = off + (uint64_t)i * bpp;          /* < 2 cap: a span is shorter than the ring */
+		return p + (q >= cap ? q - cap : q);
+	}
+};
+
+/* mixed-rate receivers: n_dec x os_r samples from the receiver's own place in the span (vdl2_rx_span_offset) */
+struct k0_rows_mixed {
+	const uint8_t *raw0; uint32_t n_dec_p; const vdl2_rx_input *rx; const vdl2_chunk_args *ca;
+	__device__ uint32_t n_dec() const { return ca ? ca->n_pairs : n_dec_p; }
+	__device__ uint32_t count(const vdl2_rx_input &in) const { return n_dec() * in.oversample; }
+	__device__ k0_run row() const { return { (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec()) }; }
+};
+
+/* ragged spans: the span[r].n x os_r samples receiver r brought to this span, at its entry of the span's receiver table */
+struct k0_rows_ragged {
+	const uint8_t *raw0; const vdl2_rx_span *span; const vdl2_chunk_args *ca;
+	__device__ uint32_t count(const vdl2_rx_input &in) const { return span[blockIdx.y].n * in.oversample; }
+	__device__ k0_run row() const { return { (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + span[blockIdx.y].off }; }
+};
+
+/* pushed spans: the span[r].n x os_r samples of receiver r where its pushes left them, in its ring (ring[r]) from ring
+ * offset span[r].off on */
+struct k0_rows_rings {
+	const uint8_t *rings; const vdl2_rx_ring *ring; const vdl2_rx_span *span;
+	__device__ uint32_t count(const vdl2_rx_input &in) const { return span[blockIdx.y].n * in.oversample; }
+	__device__ k0_ring_run row() const { return { rings + ring[blockIdx.y].base, span[blockIdx.y].off, ring[blockIdx.y].cap }; }
+};
+
+/* sample i of a row in format fmt (0 cu8, else interleaved cs16): the float pair, and the raw codes in vi / vq */
+template<typename ROW>
+__device__ __forceinline__ float2 k0_row_sample(const ROW &row, uint32_t i, uint32_t fmt, const float *__restrict__ levels,
+		int32_t &vi, int32_t &vq) {
+	if(fmt == 0) {                                       /* src/demod.c:343-345, table from :349-354 */
+		uchar2 v = *reinterpret_cast<const uchar2 *>(row.at(i, 2u));
 		vi = v.x; vq = v.y;
 		return make_float2(__ldg(&levels[v.x]), __ldg(&levels[v.y]));
 	}
+	/* src/demod.c:361-363.  A cs16 buffer after a cu8 one of odd length starts 2 bytes off a 4-byte boundary: two 16-bit
+	 * loads then */
+	const uint8_t *p = row.at(i, 4u);
 	short2 v;
-	if((reinterpret_cast<uintptr_t>(raw) & 3u) == 0) v = reinterpret_cast<const short2 *>(raw)[i];
-	else { const short *s = reinterpret_cast<const short *>(raw) + 2u * i; v = make_short2(s[0], s[1]); }
+	if((reinterpret_cast<uintptr_t>(p) & 3u) == 0) v = *reinterpret_cast<const short2 *>(p);
+	else { const short *s = reinterpret_cast<const short *>(p); v = make_short2(s[0], s[1]); }
 	vi = v.x; vq = v.y;
 	return make_float2(__fdiv_rn((float)v.x, 32768.0f), __fdiv_rn((float)v.y, 32768.0f));
 }
 
-/* levels form of the per-receiver rows: block b of row r converts samples [b, b + 1) x 256 K0_LV_SPT of the row's n
- * samples, sample i at byte offset at(i) of raw, into out[i], and counts them into acc */
-template<typename AT>
-__device__ __forceinline__ void k0_row_levels(const uint8_t *__restrict__ raw, const vdl2_rx_input &in, uint32_t n, AT at,
-		const float *__restrict__ levels, float2 *__restrict__ out, vdl2_levels *__restrict__ acc) {
-	k0_level_part t = k0_level_zero();
+/* the row body: the plain form converts one sample per thread; the levels form has block b convert samples [b, b + 1) x
+ * 256 K0_LV_SPT of the row and count them into lv[r] */
+template<bool LEVELS, typename ROWS>
+__device__ __forceinline__ void k0_convert_row(const ROWS &rows, const vdl2_rx_input *__restrict__ rx, const float *__restrict__ levels,
+		float2 *__restrict__ out0, uint32_t out_stride, vdl2_levels *__restrict__ lv) {
+	const vdl2_rx_input in = rx[blockIdx.y];
+	float2 *out = out0 + (size_t)blockIdx.y * out_stride;
+	int32_t vi, vq;
+	if constexpr(!LEVELS) {
+		const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+		if(i >= rows.count(in)) return;
+		out[i] = k0_row_sample(rows.row(), i, in.fmt, levels, vi, vq);
+	} else {
+		const uint32_t n = rows.count(in);
+		if(blockIdx.x * 256u * K0_LV_SPT >= n) return;      /* (uniform over the block) */
+		const auto row = rows.row();
+		k0_level_part t = k0_level_zero();
 #pragma unroll 4
-	for(uint32_t k = 0; k < K0_LV_SPT; k++) {
-		const uint32_t i = (blockIdx.x * K0_LV_SPT + k) * 256u + threadIdx.x;
-		if(i >= n) break;
-		int32_t vi, vq;
-		out[i] = k0_mixed_sample_raw(raw + at(i), in, 0, levels, vi, vq);
-		k0_level_add(t, in.fmt, vi, vq);
+		for(uint32_t k = 0; k < K0_LV_SPT; k++) {
+			const uint32_t i = (blockIdx.x * K0_LV_SPT + k) * 256u + threadIdx.x;
+			if(i >= n) break;
+			out[i] = k0_row_sample(row, i, in.fmt, levels, vi, vq);
+			k0_level_add(t, in.fmt, vi, vq);
+		}
+		k0_levels_block(lv + blockIdx.y, t);
 	}
-	k0_levels_block(acc, t);
 }
 
 template<bool LEVELS>
 __global__ void __launch_bounds__(256) k0_convert_mixed(const uint8_t *__restrict__ raw0, uint32_t n_dec_p, const vdl2_rx_input *__restrict__ rx,
 		const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride, const vdl2_chunk_args *__restrict__ ca,
 		vdl2_levels *__restrict__ lv) {
-	const uint32_t n_dec = ca ? ca->n_pairs : n_dec_p;
-	const vdl2_rx_input in = rx[blockIdx.y];
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if constexpr(!LEVELS) {
-	if(i >= n_dec * in.oversample) return;
-	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec);
-	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(raw, in, i, levels);
-	} else {
-		const uint32_t n = n_dec * in.oversample;
-		if(blockIdx.x * 256u * K0_LV_SPT >= n) return;      /* (uniform over the block) */
-		const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + vdl2_rx_span_offset(rx, blockIdx.y, n_dec);
-		const uint32_t bpp = in.fmt == 0 ? 2u : 4u;
-		k0_row_levels(raw, in, n, [bpp](uint32_t j) { return (size_t)j * bpp; }, levels, out0 + (size_t)blockIdx.y * out_stride, lv + blockIdx.y);
-	}
+	k0_convert_row<LEVELS>(k0_rows_mixed{ raw0, n_dec_p, rx, ca }, rx, levels, out0, out_stride, lv);
 }
 
-/* K0 on ragged spans: grid row r converts the span[r].n x os_r samples receiver r brought to this span, from its own place
- * in the span (its entry of the span's receiver table), into row r of the sample plane; rows past their count idle */
 template<bool LEVELS>
 __global__ void __launch_bounds__(256) k0_convert_ragged(const uint8_t *__restrict__ raw0, const vdl2_rx_input *__restrict__ rx,
 		const vdl2_rx_span *__restrict__ span, const float *__restrict__ levels, float2 *__restrict__ out0, uint32_t out_stride,
 		const vdl2_chunk_args *__restrict__ ca, vdl2_levels *__restrict__ lv) {
-	const vdl2_rx_input in = rx[blockIdx.y];
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if constexpr(!LEVELS) {
-	if(i >= span[blockIdx.y].n * in.oversample) return;
-	const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + span[blockIdx.y].off;
-	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(raw, in, i, levels);
-	} else {
-		const uint32_t n = span[blockIdx.y].n * in.oversample;
-		if(blockIdx.x * 256u * K0_LV_SPT >= n) return;      /* (uniform over the block) */
-		const uint8_t *raw = (ca ? static_cast<const uint8_t *>(ca->raw) : raw0) + span[blockIdx.y].off;
-		const uint32_t bpp = in.fmt == 0 ? 2u : 4u;
-		k0_row_levels(raw, in, n, [bpp](uint32_t j) { return (size_t)j * bpp; }, levels, out0 + (size_t)blockIdx.y * out_stride, lv + blockIdx.y);
-	}
+	k0_convert_row<LEVELS>(k0_rows_ragged{ raw0, span, ca }, rx, levels, out0, out_stride, lv);
 }
 
-/* K0 on pushed spans: grid row r converts the span[r].n x os_r samples of receiver r where its pushes left them, in its
- * ring (ring[r]) from ring offset span[r].off on, wrapping at the ring's end, into row r of the sample plane.  The ring's
- * capacity is a multiple of the sample size and its tail advances in whole groups, so no sample straddles the wrap and
- * every cs16 sample starts 4-byte aligned. */
 template<bool LEVELS>
 __global__ void __launch_bounds__(256) k0_convert_rings(const uint8_t *__restrict__ rings, const vdl2_rx_input *__restrict__ rx,
 		const vdl2_rx_ring *__restrict__ ring, const vdl2_rx_span *__restrict__ span, const float *__restrict__ levels,
 		float2 *__restrict__ out0, uint32_t out_stride, vdl2_levels *__restrict__ lv) {
-	const vdl2_rx_input in = rx[blockIdx.y];
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if constexpr(!LEVELS) {
-	if(i >= span[blockIdx.y].n * in.oversample) return;
-	const vdl2_rx_ring rg = ring[blockIdx.y];
-	uint64_t p = span[blockIdx.y].off + (uint64_t)i * (in.fmt == 0 ? 2u : 4u);     /* < 2 cap: a span is shorter than the ring */
-	if(p >= rg.cap) p -= rg.cap;
-	out0[(size_t)blockIdx.y * out_stride + i] = k0_mixed_sample(rings + rg.base + p, in, 0, levels);
-	} else {
-		const uint32_t n = span[blockIdx.y].n * in.oversample;
-		if(blockIdx.x * 256u * K0_LV_SPT >= n) return;      /* (uniform over the block) */
-		const vdl2_rx_ring rg = ring[blockIdx.y];
-		const uint64_t off = span[blockIdx.y].off, cap = rg.cap;
-		const uint32_t bpp = in.fmt == 0 ? 2u : 4u;
-		k0_row_levels(rings + rg.base, in, n, [off, cap, bpp](uint32_t j) {
-			uint64_t p = off + (uint64_t)j * bpp;               /* < 2 cap: a span is shorter than the ring */
-			return p >= cap ? p - cap : p;
-		}, levels, out0 + (size_t)blockIdx.y * out_stride, lv + blockIdx.y);
-	}
+	k0_convert_row<LEVELS>(k0_rows_rings{ rings, ring, span }, rx, levels, out0, out_stride, lv);
 }
 
 /* ------------------------------------------------------------------------------------------------
@@ -1784,33 +1774,23 @@ extern "C" int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t 
 	return (int)cudaGetLastError();
 }
 
-extern "C" int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *rx, uint32_t n_rx, uint32_t os_max, const float *levels,
-		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st) {
-	if(n_dec == 0 || n_rx == 0) return 0;
-	const uint32_t per_block = lv ? 256u * K0_LV_SPT : 256u;
-	auto k = lv ? k0_convert_mixed<true> : k0_convert_mixed<false>;
-	k<<<dim3((n_dec * os_max + per_block - 1) / per_block, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), n_dec, rx, levels,
-			reinterpret_cast<float2 *>(out2), out_stride, ca, lv);
-	return (int)cudaGetLastError();
-}
-
-extern "C" int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
-		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st) {
+extern "C" int vdl2_launch_k0_rows(const vdl2_k0_rows *r, uint32_t width, uint32_t n_rx, uint32_t os_max, const float *levels, float *out2,
+		uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st) {
 	if(width == 0 || n_rx == 0) return 0;
 	const uint32_t per_block = lv ? 256u * K0_LV_SPT : 256u;
-	auto k = lv ? k0_convert_ragged<true> : k0_convert_ragged<false>;
-	k<<<dim3((width * os_max + per_block - 1) / per_block, n_rx), 256, 0, st>>>(static_cast<const uint8_t *>(raw), rx, span, levels,
-			reinterpret_cast<float2 *>(out2), out_stride, ca, lv);
-	return (int)cudaGetLastError();
-}
-
-extern "C" int vdl2_launch_k0_rings(const uint8_t *rings, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_ring *ring, const vdl2_rx_span *span,
-		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, vdl2_levels *lv, cudaStream_t st) {
-	if(width == 0 || n_rx == 0) return 0;
-	const uint32_t per_block = lv ? 256u * K0_LV_SPT : 256u;
-	auto k = lv ? k0_convert_rings<true> : k0_convert_rings<false>;
-	k<<<dim3((width * os_max + per_block - 1) / per_block, n_rx), 256, 0, st>>>(rings, rx, ring, span, levels,
-			reinterpret_cast<float2 *>(out2), out_stride, lv);
+	const dim3 grid((width * os_max + per_block - 1) / per_block, n_rx);
+	const uint8_t *raw = static_cast<const uint8_t *>(r->raw);
+	float2 *out = reinterpret_cast<float2 *>(out2);
+	if(r->ring) {
+		auto k = lv ? k0_convert_rings<true> : k0_convert_rings<false>;
+		k<<<grid, 256, 0, st>>>(raw, r->rx, r->ring, r->span, levels, out, out_stride, lv);
+	} else if(r->span) {
+		auto k = lv ? k0_convert_ragged<true> : k0_convert_ragged<false>;
+		k<<<grid, 256, 0, st>>>(raw, r->rx, r->span, levels, out, out_stride, ca, lv);
+	} else {
+		auto k = lv ? k0_convert_mixed<true> : k0_convert_mixed<false>;
+		k<<<grid, 256, 0, st>>>(raw, width, r->rx, levels, out, out_stride, ca, lv);
+	}
 	return (int)cudaGetLastError();
 }
 

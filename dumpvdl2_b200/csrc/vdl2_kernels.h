@@ -167,18 +167,22 @@ int vdl2_launch_k0(const void *raw, uint32_t n_pairs, uint32_t fmt, const float 
 /* one stream per channel: raw[s][i] -> out2[i][out_stride] float2, time-major across streams */
 int vdl2_launch_k0_lanes(const void *raw, uint32_t n_pairs, uint32_t fmt, const float *levels, float *out2, uint32_t n_streams,
 		uint32_t raw_stride, uint32_t out_stride, uint32_t lanes, uint32_t full_warps, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
-/* mixed-rate receivers: row r converts n_dec x rx[r].oversample samples in format rx[r].fmt from raw + n_dec x
- * rx[r].off_per_dec into out2 + r x out_stride float2 (n_dec from ca->n_pairs when ca is given) */
-int vdl2_launch_k0_mixed(const void *raw, uint32_t n_dec, const vdl2_rx_input *rx, uint32_t n_rx, uint32_t os_max, const float *levels,
-		float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
-/* ragged spans: row r converts span[r].n x rx[r].oversample samples from raw + span[r].off; width = the largest span[r].n
- * (sizes the grid) */
-int vdl2_launch_k0_ragged(const void *raw, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_span *span, uint32_t n_rx, uint32_t os_max,
-		const float *levels, float *out2, uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
-/* pushed spans: row r converts span[r].n x rx[r].oversample samples from receiver r's ring (rings + ring[r].base), starting
- * at ring offset span[r].off and wrapping at ring[r].cap; width = the largest span[r].n (sizes the grid) */
-int vdl2_launch_k0_rings(const uint8_t *rings, uint32_t width, const vdl2_rx_input *rx, const vdl2_rx_ring *ring, const vdl2_rx_span *span,
-		uint32_t n_rx, uint32_t os_max, const float *levels, float *out2, uint32_t out_stride, vdl2_levels *lv, cudaStream_t st);
+/* one row per receiver: row r converts its samples, in format rx[r].fmt, into out2 + r x out_stride float2.  The row
+ * source is the first of these that applies:
+ *   pushed spans (ring given): span[r].n x rx[r].oversample samples from receiver r's ring (raw + ring[r].base), starting at
+ *     ring offset span[r].off and wrapping at ring[r].cap;
+ *   ragged spans (span given): span[r].n x rx[r].oversample samples from raw + span[r].off;
+ *   mixed-rate receivers: width x rx[r].oversample samples from raw + width x rx[r].off_per_dec.
+ * width: the largest span[r].n, or the mixed span's decimated samples (sizes the grid).  When ca is given, mixed and
+ * ragged rows take raw from ca->raw, and mixed rows their decimated samples from ca->n_pairs. */
+typedef struct {
+	const void *raw;             /* the span's bytes, or (pushed spans) the receivers' rings */
+	const vdl2_rx_input *rx;
+	const vdl2_rx_span *span;    /* ragged and pushed spans, else NULL */
+	const vdl2_rx_ring *ring;    /* pushed spans, else NULL */
+} vdl2_k0_rows;
+int vdl2_launch_k0_rows(const vdl2_k0_rows *r, uint32_t width, uint32_t n_rx, uint32_t os_max, const float *levels, float *out2,
+		uint32_t out_stride, const vdl2_chunk_args *ca, vdl2_levels *lv, cudaStream_t st);
 int vdl2_launch_k1(const vdl2_k1_params *p, int force_scalar, int variant, cudaStream_t st);
 int vdl2_launch_copy_hist(const vdl2_k2_params *p, cudaStream_t st);
 int vdl2_launch_k2a(const vdl2_k2_params *p, cudaStream_t st);

@@ -94,7 +94,6 @@ def main():
                 ("k2_ring_staged", dict(VDL2GPU_K2_VARIANT=5), 0), ("k1_one_warp", dict(VDL2GPU_K1_VARIANT=8), 0),
                 ("k2_staged_1warp", dict(VDL2GPU_K2_VARIANT=261), 0), ("k2_plane_1warp", dict(VDL2GPU_K2_VARIANT=258), 0),
                 ("all_1warp", dict(VDL2GPU_K2_VARIANT=261, VDL2GPU_K1_VARIANT=8), 0),
-                ("k2a_overlap", dict(VDL2GPU_K2A_EXCLUSIVE=0), 0), ("k2a_overlap_libm", dict(VDL2GPU_K2A_EXCLUSIVE=0, VDL2GPU_K2A=0), 0),
                 ("split8", dict(VDL2GPU_K2A_SPLIT=8), 0), ("split16", dict(VDL2GPU_K2A_SPLIT=16), 0), ("split32", dict(VDL2GPU_K2A_SPLIT=32), 0),
                 ("split64", dict(VDL2GPU_K2A_SPLIT=64), 0), ("stages3", dict(VDL2GPU_STAGES=3), 0),
                 ("default_again", {}, 0), ("no_graph_again", {}, vd.FLAG_NO_GRAPH)]
