@@ -18,6 +18,7 @@
 #include <stdint.h>
 #include <string.h>
 #include "vdl2_types.h"
+#include "vdl2_fastmath.cuh"
 
 /* branch layout hints: a sync decision, a noise-floor update or a lock are rare events of the walk's hot path */
 #define VDL2_UNLIKELY(x) __builtin_expect(!!(x), 0)
@@ -434,8 +435,17 @@ VDL2_HD void vdl2_burst_complete(vdl2_chan &v, const vdl2_k2_env &env, uint32_t 
  *   (float)atan2((double)im, (double)re)                 src/demod.c:232,256 (double atan2, narrowed on store)
  *   hypotf(re, im)                                       src/demod.c:238; glibc evaluates sqrt(x*x + y*y) in double and narrows
  * Both are pure functions of the sample, so the K2a pre-pass computes them for every decimated sample of the
- * chunk in parallel and the sequential state machine only consumes them. */
-VDL2_HD float vdl2_phase_of(float re, float im) { return D_TO_F(atan2((double)im, (double)re)); }
+ * chunk in parallel and the sequential state machine only consumes them.
+ * The phase is atan2 correctly rounded to double, narrowed.  On the device that is vdl2_atan2_cr (vdl2_fastmath.cuh):
+ * libdevice's double atan2 (2 ulp) narrows to the wrong float on some samples next to a float rounding boundary
+ * (tests/golden/phase_hard.json).  Host builds use glibc's atan2, which the reference uses. */
+VDL2_HD float vdl2_phase_of(float re, float im) {
+#if defined(__CUDA_ARCH__)
+	return vdl2_atan2_cr(re, im);
+#else
+	return D_TO_F(atan2((double)im, (double)re));
+#endif
+}
 VDL2_HD float vdl2_mag_of(float re, float im) {
 	return D_TO_F(D_SQRT(D_ADD(D_MUL((double)re, (double)re), D_MUL((double)im, (double)im))));
 }

@@ -9,7 +9,8 @@
  * double with a short argument reduction (9 break points k/8, one division, a degree-5 polynomial in t^2:
  * ~22 FP64 operations instead of the ~65 of the libdevice routine) and reports, Ziv style, whether its result
  * is too close to a rounding boundary to be trusted; the caller then falls back to the full routine (about one
- * sample in a million).  The float returned without the fall-back flag is the correctly rounded one.
+ * sample in a million; on the device vdl2_atan2_cr below).  The float returned without the fall-back flag is the
+ * correctly rounded one, which away from a rounding boundary is also the narrowed correctly rounded double.
  *
  * Error budget (relative to the final result r; the guard used is 2^-44, 16x the bound):
  *   t = num/den      num, den exact in double (|c| <= 1 has 4 significant bits, the floats 24);
@@ -59,7 +60,7 @@
 #define VDL2_FM_C3 0x1.999999999999ap-3    /*  1/5  */
 #define VDL2_FM_C4 -0x1.5555555555555p-2   /* -1/3  */
 #if defined(__CUDACC__)
-__constant__ double c_vdl2_fm[9] = { VDL2_FM_C0, VDL2_FM_C1, VDL2_FM_C2, VDL2_FM_C3, VDL2_FM_C4, VDL2_PIO2_HI, VDL2_PIO2_LO, VDL2_PI_HI, VDL2_PI_LO };
+static __constant__ double c_vdl2_fm[9] = { VDL2_FM_C0, VDL2_FM_C1, VDL2_FM_C2, VDL2_FM_C3, VDL2_FM_C4, VDL2_PIO2_HI, VDL2_PIO2_LO, VDL2_PI_HI, VDL2_PI_LO };
 #endif
 #if defined(__CUDA_ARCH__)
 #define VDL2_FM_K(i, v) c_vdl2_fm[i]
@@ -281,6 +282,92 @@ VDL2_FM_HD float vdl2_mag_fast_nb(float re, float im, int *slow) {
 	const uint32_t dist = drop > 0x10000000u ? drop - 0x10000000u : 0x10000000u - drop;
 	*slow = (!in_range || dist < 512u) ? 1 : 0;
 	return (float)g;
+}
+
+/* ---- the fall-back: atan2(im, re) correctly rounded to double, narrowed to float ----
+ * This is the reference's float whenever its libm's atan2 is correctly rounded (glibc's is on every sample of
+ * tests/golden/phase_hard.json).  It is not always the float nearest to atan2: within half a double ulp of a float midpoint
+ * the double is the midpoint itself and the narrowing goes to the even float (double rounding), and so does the reference.
+ * The samples that reach the fall-back are the ones next to a float midpoint, where an atan2 in double with an error of an
+ * ulp or two (libdevice documents 2) can narrow to the other float.  This routine continues the reduction of
+ * vdl2_phase_fast in double-double:
+ *   t = num/den      num, den exact; th = RN(num/den), tl = RN((num - den th)/den), the residual exact: |dt/t| <= 2^-104
+ *   atan(t)          |t| <= 1/16: the series to t^23 (truncation t^25/25 <= 2^-100 t); the terms up to t^11 with
+ *                    double-double coefficients, the rest in double (their share is below 2^-48 t)
+ *   A_k + atan(t)    atan(k/8) and the folding constants pi/2, pi as hi + lo pairs (mpmath at 200 bits)
+ *   total            below 2^-98 relative; hi of the normalised sum is the double nearest to it, so hi is the correctly
+ *                    rounded double unless atan2 lies within 2^-98 (relative) of a midpoint between two doubles
+ * About 150 double operations; the pipeline calls it for a few samples per million. */
+/* {atan(k/8) hi, lo} for k = 0..8 (mpmath at 200 bits; the hi parts are VDL2_ATAN_TABLE_INIT's) */
+#define VDL2_ATAN_DD_INIT { 0.0, 0.0, 0x1.fd5ba9aac2f6ep-4, -0x1.cd37686760c17p-59, 0x1.f5b75f92c80ddp-3, 0x1.8ab6e3cf7afbdp-57, \
+	0x1.6f61941e4def1p-2, -0x1.c63aae6f6e918p-56, 0x1.dac670561bb4fp-2, 0x1.a2b7f222f65e2p-56, 0x1.1e00babdefeb4p-1, -0x1.928df287a668fp-58, \
+	0x1.4978fa3269ee1p-1, 0x1.2419a87f2a458p-56, 0x1.700a7c5784634p-1, -0x1.8c34d25aadef6p-56, 0x1.921fb54442d18p-1, 0x1.1a62633145c07p-55 }
+#if defined(__CUDACC__)
+static __constant__ double c_vdl2_atan_dd[18] = VDL2_ATAN_DD_INIT;
+#endif
+#if defined(__CUDA_ARCH__)
+#define VDL2_ATAN_DD(i) c_vdl2_atan_dd[i]
+#else
+static const double vdl2_atan_dd_host[18] = VDL2_ATAN_DD_INIT;
+#define VDL2_ATAN_DD(i) vdl2_atan_dd_host[i]
+#endif
+
+VDL2_FM_HD void vdl2_dd_add(double ah, double al, double bh, double bl, double *rh, double *rl) {
+	const double s = ah + bh, v = s - ah;
+	const double e = ((ah - (s - v)) + (bh - v)) + (al + bl);          /* two-sum of the high parts, then the low parts */
+	*rh = s + e;
+	*rl = e - (*rh - s);
+}
+
+VDL2_FM_HD void vdl2_dd_mul(double ah, double al, double bh, double bl, double *rh, double *rl) {
+	const double p = ah * bh;
+	const double e = vdl2_fm_fma(ah, bh, -p) + (ah * bl + al * bh);   /* exact product of the high parts + cross terms */
+	*rh = p + e;
+	*rl = e - (*rh - p);
+}
+
+VDL2_FM_HD float vdl2_atan2_cr(float re, float im) {
+	if(!(fabsf(re) <= 3.4028235e38f && fabsf(im) <= 3.4028235e38f) || (re == 0.0f && im == 0.0f)) {
+		/* NaN, infinite or (+-0, +-0): the C99 results are those of the sample with each infinity made +-1 and the
+		 * finite component +-0, and of (+-1, +-0) for (+-0, +-0) */
+		if(isnan(re) || isnan(im)) return re + im;
+		const bool ri = isinf(re), ii = isinf(im);
+		re = copysignf(ri || !ii ? 1.0f : 0.0f, re);
+		im = copysignf(ii ? 1.0f : 0.0f, im);
+	}
+	const double ax = fabs((double)re), ay = fabs((double)im);
+	const double mx = fmax(ax, ay), mn = fmin(ax, ay);
+	const int k = (int)(mn / mx * 8.0 + 0.5);                           /* |t| <= 1/16 */
+	const double c = 0.125 * k;
+	const double num = vdl2_fm_fma(-c, mx, mn), den = vdl2_fm_fma(c, mn, mx);    /* exact */
+	const double th = num / den;
+	const double tl = vdl2_fm_fma(-th, den, num) / den;
+	double sh, sl;
+	vdl2_dd_mul(th, tl, th, tl, &sh, &sl);
+	/* t^13 .. t^23 in double, then t^3 .. t^11 in double-double */
+	double tail = -0x1.642c8590b2164p-5;                                 /* -1/23 */
+	tail = tail * sh + 0x1.8618618618618p-5;                             /*  1/21 */
+	tail = tail * sh - 0x1.af286bca1af28p-5;                             /* -1/19 */
+	tail = tail * sh + 0x1.e1e1e1e1e1e1ep-5;                             /*  1/17 */
+	tail = tail * sh - 0x1.1111111111111p-4;                             /* -1/15 */
+	tail = tail * sh + 0x1.3b13b13b13b14p-4;                             /*  1/13 */
+	const double ch[5] = { -0x1.745d1745d1746p-4, 0x1.c71c71c71c71cp-4, -0x1.2492492492492p-3, 0x1.999999999999ap-3, -0x1.5555555555555p-2 };
+	const double cl[5] = { 0x1.745d1745d1746p-59, 0x1.c71c71c71c71cp-58, -0x1.2492492492492p-57, -0x1.999999999999ap-57, -0x1.5555555555555p-56 };
+	double ph = tail, pl = 0.0;
+#pragma unroll
+	for(int j = 0; j < 5; j++) {                                         /* p = p s + (-1)^j / (2j + 1), j = 5 .. 1 */
+		vdl2_dd_mul(ph, pl, sh, sl, &ph, &pl);
+		vdl2_dd_add(ph, pl, ch[j], cl[j], &ph, &pl);
+	}
+	double rh, rl;
+	vdl2_dd_mul(ph, pl, sh, sl, &ph, &pl);                              /* atan t = t + t (s p) */
+	vdl2_dd_mul(th, tl, ph, pl, &ph, &pl);
+	vdl2_dd_add(th, tl, ph, pl, &rh, &rl);
+	vdl2_dd_add(VDL2_ATAN_DD(2 * k), VDL2_ATAN_DD(2 * k + 1), rh, rl, &rh, &rl);
+	if(ay > ax) vdl2_dd_add(VDL2_PIO2_HI, VDL2_PIO2_LO, -rh, -rl, &rh, &rl);
+	if(re < 0.0f) vdl2_dd_add(VDL2_PI_HI, VDL2_PI_LO, -rh, -rl, &rh, &rl);
+	const float f = (float)rh;
+	return copysignf(f, im);
 }
 
 #endif

@@ -2145,7 +2145,7 @@ extern "C" int vdl2gpu_launch_rs_verify(uint8_t *blocks, const int32_t *fec_octe
 
 /* K2a on its own: phase_out[i] = (float)atan2((double)im, (double)re), mag_out[i] = hypotf(re, im) of n_elems
  * decimated samples (src/demod.c:232,238,256).  exact_libm = 0: the Ziv-guarded short evaluation the pipeline
- * uses (vdl2_fastmath.cuh); 1: the libdevice routine for every element.  Both give the same floats. */
+ * uses (vdl2_fastmath.cuh); 1: vdl2_phase_of / vdl2_mag_of for every element (no fast path).  Both give the same floats. */
 extern "C" int vdl2gpu_launch_phase_mag(const float *dec, uint32_t n_elems, float *phase_out, float *mag_out, int exact_libm, void *stream) {
 	if(n_elems && (!dec || !phase_out || !mag_out)) return VDL2GPU_EINVAL;
 	if(n_elems == 0) return VDL2GPU_OK;

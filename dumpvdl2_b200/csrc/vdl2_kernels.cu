@@ -1041,8 +1041,8 @@ __global__ void __launch_bounds__(VDL2_RX_K1_BLOCK) k1_mix_iir_decimate_ragged(v
  * FAST: the phase comes from vdl2_phase_fast (vdl2_fastmath.cuh: 9 break points, one division, degree-5 polynomial,
  * ~22 FP64 operations) whose float result is the correctly rounded fl32(atan2), the magnitude from vdl2_mag_fast
  * (exact sum of squares, Newton square root); only when one of them reports that its double lies within 2^-44 of a
- * float rounding boundary, or for zero / non-finite / extreme inputs (about one sample in 3e5), the libdevice
- * routine / the IEEE square root decide, as they do for every sample when FAST is off. */
+ * float rounding boundary, or for zero / non-finite / extreme inputs (about one sample in 3e5), vdl2_phase_of (the
+ * double-double vdl2_atan2_cr) / the IEEE square root decide, as they do for every sample when FAST is off. */
 
 template<bool FAST>
 __global__ void __launch_bounds__(256) k2a_phase_mag(const float2 *__restrict__ dec, float *__restrict__ phase,
@@ -1194,7 +1194,7 @@ __device__ __forceinline__ void k2a_warps_body(const vdl2_k2a_params &p) {
 }
 
 template<bool FAST, bool LEVELS>
-__global__ void __launch_bounds__(128, LEVELS ? 6 : 8) k2a_phase_mag_warps(vdl2_k2a_params p) { k2a_warps_body<FAST, false, LEVELS>(p); }     /* <= 64 registers: 32 warps per SM */
+__global__ void __launch_bounds__(128, LEVELS ? 6 : FAST ? 7 : 8) k2a_phase_mag_warps(vdl2_k2a_params p) { k2a_warps_body<FAST, false, LEVELS>(p); }     /* FAST: <= 72 registers, 28 warps per SM (the fall-back spills at 64); else <= 64: 32 warps */
 /* (the lane's own row count and slice end take two more registers than the uniform ones of the lock-step kernel: within 64
  * the fast form spilled, so seven blocks per SM, <= 72 registers) */
 template<bool FAST, bool LEVELS>

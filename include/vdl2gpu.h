@@ -513,8 +513,9 @@ int vdl2gpu_launch_rs_verify(uint8_t *blocks /* [n][255] */, const int32_t *fec_
 		int32_t *ret_out, void *stream);
 
 /* K2a: phase_out[i] = (float)atan2((double)im, (double)re) and mag_out[i] = hypotf(re, im) of n_elems decimated
- * samples dec[n_elems][2] (src/demod.c:232,238,256).  exact_libm = 0: the short double-precision evaluation with a
- * Ziv rounding test the pipeline uses; 1: the general libdevice atan2 for every element.  Same floats either way. */
+ * samples dec[n_elems][2] (src/demod.c:232,238,256); the phase is atan2 correctly rounded to double, narrowed.
+ * exact_libm = 0: the short double-precision evaluation with a Ziv rounding test the pipeline uses, and the full
+ * evaluation where that test fails; 1: the full evaluation for every element (no fast path).  Same floats either way. */
 int vdl2gpu_launch_phase_mag(const float *dec, uint32_t n_elems, float *phase_out, float *mag_out, int exact_libm, void *stream);
 
 /* ---- stage stubs: the three per-channel stages one at a time, on device memory the caller owns.
