@@ -42,6 +42,34 @@ static int fail_cuda(cudaError_t e, const char *what, int line) {
 #define CU(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) return fail_cuda(e_, #call, __LINE__); } while(0)
 #define KL(call) do { int e_ = (call); if(e_ != 0) return fail_cuda((cudaError_t)e_, #call, __LINE__); } while(0)
 
+/* One owner per CUDA resource: a handle releases what it holds when it is reset, moved onto or destroyed, and a null
+ * handle releases nothing.  It reads as the raw handle; put() releases the old one and hands a creating call the address
+ * to fill, as in CU(cudaMalloc(x.put(), bytes)). */
+template<typename T, typename Release>
+class owned {
+	T h_ = nullptr;
+public:
+	owned() = default;
+	owned(owned &&o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+	owned &operator=(owned &&o) noexcept { if(this != &o) { reset(); h_ = o.h_; o.h_ = nullptr; } return *this; }
+	~owned() { reset(); }
+	void reset() { if(h_) Release()(h_); h_ = nullptr; }
+	T *put() { reset(); return &h_; }
+	T get() const { return h_; }
+	operator T() const { return h_; }
+	T operator->() const { return h_; }
+};
+struct free_dev { void operator()(void *p) const { cudaFree(p); } };
+struct free_host { void operator()(void *p) const { cudaFreeHost(p); } };
+struct destroy_event { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct destroy_stream { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+struct destroy_graph_exec { void operator()(cudaGraphExec_t g) const { cudaGraphExecDestroy(g); } };
+template<typename T> using dev_mem = owned<T *, free_dev>;
+template<typename T> using host_mem = owned<T *, free_host>;          /* cudaHostAlloc */
+using event_h = owned<cudaEvent_t, destroy_event>;
+using stream_h = owned<cudaStream_t, destroy_stream>;
+using graph_exec_h = owned<cudaGraphExec_t, destroy_graph_exec>;
+
 /* ------------------------------------------------------------------------------------------------
  * context
  * ---------------------------------------------------------------------------------------------- */
@@ -52,29 +80,29 @@ struct pending_frame {
 };
 
 struct chunk_slot {
-	uint8_t *h_raw = nullptr, *d_raw = nullptr;
-	uint8_t *h_out = nullptr, *d_out = nullptr;
-	cudaEvent_t done = nullptr;
-	cudaEvent_t tk[8] = { nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr };   /* front: 0,1,2  mid: 3,6  back: 7,4,5 */
+	host_mem<uint8_t> h_raw; dev_mem<uint8_t> d_raw;
+	host_mem<uint8_t> h_out; uint8_t *d_out = nullptr;  /* mapped: d_out is h_out's device address */
+	event_h done;
+	event_h tk[8];                                      /* front: 0,1,2  mid: 3,6  back: 7,4,5 */
 	bool busy = false, timed = false;
 	uint64_t seq = 0;
 	/* per-chunk arguments (pinned host copy, device copy made by the first node of the front graph) and the three
 	 * CUDA graphs of this slot per decimated-sample buffer: front {args copy, K0, K1}, K2a, back {K2, history, K3, finish} */
-	vdl2_chunk_args *h_args = nullptr, *d_args = nullptr;
+	host_mem<vdl2_chunk_args> h_args; dev_mem<vdl2_chunk_args> d_args;
 	/* ragged spans: the span's receiver table (vdl2_rx_span_table; pinned host copy, device copy made with the arguments) */
-	vdl2_rx_span *h_span = nullptr, *d_span = nullptr;
+	host_mem<vdl2_rx_span> h_span; dev_mem<vdl2_rx_span> d_span;
 	/* ragged spans that restart receivers (vdl2gpu_restart_receiver): per channel slot, whether it starts afresh with this
 	 * span and its new tuning (pinned host copy, device copy made with the span's table); such a span takes the direct
 	 * path, so the graphs of ordinary spans never see the table */
-	vdl2_rx_restart *h_restart = nullptr, *d_restart = nullptr;
+	host_mem<vdl2_rx_restart> h_restart; dev_mem<vdl2_rx_restart> d_restart;
 	bool restart = false;
 	/* pushed spans (vdl2gpu_submit_pushed): K0 reads the receivers' rings; k0_done is recorded after it (ragged contexts) */
 	bool pushed = false;
-	cudaEvent_t k0_done = nullptr;
+	event_h k0_done;
 	/* spectrum (VDL2GPU_FLAG_SPECTRUM): per input, the samples it holds and brings to this chunk (pinned host copy, device
 	 * copy made right before the spectrum kernel) */
-	vdl2_spec_span *h_spec = nullptr, *d_spec = nullptr;
-	cudaGraphExec_t g_front[6] = { nullptr }, g_k2a[6] = { nullptr }, g_back[6] = { nullptr };    /* index = chunk number mod 6 (dec buffer, plane) */
+	host_mem<vdl2_spec_span> h_spec; dev_mem<vdl2_spec_span> d_spec;
+	graph_exec_h g_front[6], g_k2a[6], g_back[6];      /* index = chunk number mod 6 (dec buffer, plane) */
 	uint32_t graph_pairs[6] = { 0 };
 	uint64_t first_pair = 0, dec_base = 0;
 	uint32_t n_pairs = 0, n_dec = 0;
@@ -95,44 +123,36 @@ struct push_rx {
 	std::deque<span_anchor> anchors;                    /* (control thread only) */
 };
 
-struct vdl2gpu_ctx {
-	vdl2gpu_config cfg;
+/* the pushed-input rings of one receiver list (ragged contexts, allocated by the first vdl2gpu_push): the receivers' rings
+ * (vdl2_push_ring_layout) in device memory, their pinned host mirror and table, and per receiver its queue state */
+struct push_rings {
+	dev_mem<uint8_t> d_rings;
+	host_mem<uint8_t> h_rings;
+	std::vector<vdl2_rx_ring> rings;
+	dev_mem<vdl2_rx_ring> d_ring_tab;
+	std::vector<std::unique_ptr<push_rx>> push;
+};
+
+/* The part of a context that follows from its channels and receivers (setup_layout): vdl2gpu_update_receivers builds a new
+ * one and swaps it in whole. */
+struct ctx_layout {
 	std::vector<uint32_t> freqs;
-	int device = 0;
-	/* `stream` (front) carries H2D + K0 + K1 of chunk c+1 while `s_back` carries K2a/K2/K3 of chunk c.  Both stages
-	 * are latency-bound with one warp per SM sub-partition at 16 k channels, so co-residency raises issue-slot use.
-	 * This only works because every kernel of the chain requests the SAME
-	 * shared-memory carve-out (vdl2_kernels.cu): with per-kernel defaults the SMs drain to re-partition L1/shared
-	 * memory and the overlap is a 1.7x slow-down.  VDL2GPU_FLAG_NO_OVERLAP puts everything on one stream. */
-	cudaStream_t stream = nullptr, s_mid = nullptr, s_back = nullptr;
-	/* three stages, three chunks in flight: K0+K1 of chunk c+2 (front), K2a of chunk c+1 (mid), K2+K3 of chunk c (back).
-	 * dec is triple-buffered (written by K1, read by K2a and K2), the phase / magnitude planes alternate (written by K2a,
-	 * read by K2; K2a of chunk c takes its 160 history rows from the other plane, i.e. from chunk c-1). */
-	cudaEvent_t ev_k1_done[3] = { nullptr, nullptr, nullptr }, ev_back_done[3] = { nullptr, nullptr, nullptr }, ev_k2a_done[2] = { nullptr, nullptr };
-	uint64_t chunk_seq = 0;
-	cudaEvent_t ev_input_ready = nullptr, ev_input_consumed = nullptr;
-	uint32_t n_ch = 0, n_chp = 0, max_pairs = 0, max_dec = 0, n_slots = 0, out_cap = 0, event_cap = 0;
-	uint64_t events_dropped = 0;                        /* trace events lost to a full buffer, not yet reported by vdl2gpu_read_events */
-	uint32_t lanes = 32, full_warps = 0xFFFFFFFFu;      /* channel slot mapping (see create_impl) */
-	int n_sms = 0;                                      /* read from the device at create */
-	uint32_t n_streams = 1, ch_per_stream = 0;          /* independent-streams mode: n_streams > 1, channels [s*C, (s+1)*C) on stream s */
-	bool lane_streams = false;                          /* C == 1: samples kept time-major across streams, one lane per stream in K1 */
-	bool receivers = false;                             /* vdl2gpu_create_receivers: n_streams receivers, each with its own centre and channels */
-	uint32_t *d_slot_rx = nullptr, *d_block_rx = nullptr;   /* receivers: vdl2_rx_layout tables (fixed at create) */
+	uint32_t n_ch = 0, n_chp = 0, max_pairs = 0, max_dec = 0, n_slots = 0, out_cap = 0;
+	uint32_t lanes = 32, full_warps = 0xFFFFFFFFu;      /* channel slot mapping (see setup_layout) */
+	uint32_t n_streams = 1;                             /* inputs: streams, or receivers */
+	dev_mem<uint32_t> d_slot_rx, d_block_rx;            /* receivers: vdl2_rx_layout tables */
 	uint32_t rx_tile = 0, rx_max = 0;                   /* receivers: samples per staged tile, most receivers of one K1 block */
 	/* mixed-rate receivers (vdl2gpu_create_mixed_receivers): every receiver has its own oversample factor and format, and
 	 * the chain counts DECIMATED samples (n_pairs of a chunk = n_dec of a span, decimation counter always 0); rx_tile is
 	 * then the decimation groups of a staged tile */
-	bool mixed = false;
 	std::vector<vdl2_rx_input> rx_in;                   /* per receiver: oversample, format, byte offset per decimated sample */
-	vdl2_rx_input *d_rx_in = nullptr;
-	uint8_t *d_slot_cls = nullptr;                      /* slot -> rate class (vdl2_rx_class) of its receiver */
+	dev_mem<vdl2_rx_input> d_rx_in;
+	dev_mem<uint8_t> d_slot_cls;                        /* slot -> rate class (vdl2_rx_class) of its receiver */
 	uint64_t span_bytes_per_dec = 0, span_pairs_per_dec = 0;   /* sums over the receivers of os x bytes per sample, of os */
 	uint32_t max_span = 0, rx_os_max = 0, cls_mask = 0;  /* largest n_dec of a span; largest oversample; rate classes present */
 	float cls_taps[3][5] = {};                          /* {a0, a1, a2, b1, b2} per rate class (10, 13, 20) */
 	/* ragged spans (VDL2GPU_FLAG_RAGGED on a mixed context): every receiver brings its own count n_r to a span; the chain then
 	 * counts the span's width (the largest n_r) and each kernel lane takes its receiver's entry of the span's table */
-	bool ragged = false;
 	std::vector<uint64_t> rx_pos;                       /* per receiver: decimated samples accepted so far */
 	std::vector<uint32_t> rx_prev;                      /* per receiver: its count in the previous span */
 	std::vector<uint32_t> ch_rx;                        /* per channel: its receiver (burst timestamps) */
@@ -141,6 +161,57 @@ struct vdl2gpu_ctx {
 	std::vector<uint32_t> rx_centre, rx_first;
 	std::vector<uint8_t> rx_restart_pending;
 	uint32_t n_restart_pending = 0;
+	dev_mem<float2> d_samples;
+	dev_mem<float2> d_dec3[3];
+	dev_mem<float> d_phase2[2], d_mag2[2];
+	dev_mem<uint32_t> d_k1, d_k2, d_counters, d_ready;
+	dev_mem<float> d_ring;
+	dev_mem<vdl2_burst_slot> d_pool;
+	dev_mem<int32_t> d_free;
+	dev_mem<vdl2_queue_ctl> d_ctl;
+	/* input levels (VDL2GPU_FLAG_INPUT_LEVELS; NULL otherwise): one accumulator per input (stream or receiver), which the
+	 * levels form of K0 adds every converted sample to */
+	dev_mem<vdl2_levels> d_levels;
+	/* channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS; NULL otherwise): the per-slot planes the levels form of K2a adds every
+	 * decimated sample to, uint64 [VDL2_CHLV_ROWS][n_chp] then the uint32 peak plane [n_chp] */
+	dev_mem<uint64_t> d_chlv;
+	/* spectrum (VDL2GPU_FLAG_SPECTRUM; NULL / empty otherwise): per input its accumulators and waiting samples, the window and
+	 * twiddle tables, and per input its position on its segment grid (samples since the grid's origin: create, joining,
+	 * restart); inputs whose figures a restart zeroes at the start of the next span */
+	dev_mem<vdl2_spec_acc> d_spec;
+	dev_mem<vdl2_spec_tab> d_spec_tab;
+	std::vector<uint64_t> spec_pos;
+	std::vector<uint32_t> spec_zero;
+	std::vector<chunk_slot> chunks;
+};
+
+struct vdl2gpu_ctx : ctx_layout, push_rings {
+	/* the config create was given, max_chunk_bytes and n_inflight defaulted; its channel fields (freqs, n_channels,
+	 * n_streams) are create's input only: the layout holds the current ones */
+	vdl2gpu_config cfg;
+	int device = 0;
+	/* `stream` (front) carries H2D + K0 + K1 of chunk c+1 while `s_back` carries K2a/K2/K3 of chunk c.  Both stages
+	 * are latency-bound with one warp per SM sub-partition at 16 k channels, so co-residency raises issue-slot use.
+	 * This only works because every kernel of the chain requests the SAME
+	 * shared-memory carve-out (vdl2_kernels.cu): with per-kernel defaults the SMs drain to re-partition L1/shared
+	 * memory and the overlap is a 1.7x slow-down.  VDL2GPU_FLAG_NO_OVERLAP puts everything on one stream.
+	 * s_back and s_mid alias `stream`, back_stream or mid_stream, whichever create made for them. */
+	stream_h stream, back_stream, mid_stream;
+	cudaStream_t s_mid = nullptr, s_back = nullptr;
+	/* three stages, three chunks in flight: K0+K1 of chunk c+2 (front), K2a of chunk c+1 (mid), K2+K3 of chunk c (back).
+	 * dec is triple-buffered (written by K1, read by K2a and K2), the phase / magnitude planes alternate (written by K2a,
+	 * read by K2; K2a of chunk c takes its 160 history rows from the other plane, i.e. from chunk c-1). */
+	event_h ev_k1_done[3], ev_back_done[3], ev_k2a_done[2];
+	uint64_t chunk_seq = 0;
+	event_h ev_input_ready, ev_input_consumed;
+	uint32_t event_cap = 0;
+	uint64_t events_dropped = 0;                        /* trace events lost to a full buffer, not yet reported by vdl2gpu_read_events */
+	int n_sms = 0;                                      /* read from the device at create */
+	uint32_t ch_per_stream = 0;                         /* independent-streams mode: n_streams > 1, channels [s*C, (s+1)*C) on stream s */
+	bool lane_streams = false;                          /* C == 1: samples kept time-major across streams, one lane per stream in K1 */
+	bool receivers = false;                             /* vdl2gpu_create_receivers: n_streams receivers, each with its own centre and channels */
+	bool mixed = false;                                 /* vdl2gpu_create_mixed_receivers (see ctx_layout) */
+	bool ragged = false;                                /* VDL2GPU_FLAG_RAGGED (see ctx_layout) */
 	uint32_t raw_bytes = 0;                             /* size of each slot's raw staging buffers (allocated on the first host submit) */
 	int k1_variant = 2, k2_variant = 5, k2a_mode = 1;   /* A/B knobs (VDL2GPU_K1_VARIANT, VDL2GPU_K2_VARIANT, VDL2GPU_K2A), read at create */
 	bool use_graphs = true;
@@ -149,17 +220,8 @@ struct vdl2gpu_ctx {
 	                                                     * 3: K2a of chunk c+1 beside K1 of chunk c+2 and K2 of chunk c (VDL2GPU_STAGES=3) */
 	uint64_t overflows_reported = 0;
 	host_tables tab;
-	vdl2_tables *d_tab = nullptr;
-	float2 *d_samples = nullptr;
-	float2 *d_dec3[3] = { nullptr, nullptr, nullptr };
-	float *d_phase2[2] = { nullptr, nullptr }, *d_mag2[2] = { nullptr, nullptr };
-	uint32_t *d_k1 = nullptr, *d_k2 = nullptr, *d_counters = nullptr, *d_ready = nullptr;
-	float *d_ring = nullptr;
-	vdl2_burst_slot *d_pool = nullptr;
-	int32_t *d_free = nullptr;
-	vdl2_queue_ctl *d_ctl = nullptr;
-	void *d_events = nullptr;
-	std::vector<chunk_slot> chunks;
+	dev_mem<vdl2_tables> d_tab;
+	dev_mem<vdl2gpu_event> d_events;
 	std::deque<uint32_t> inflight;
 	uint32_t next_slot = 0;
 	uint32_t decim_cnt = 0, last_n_dec = 0;
@@ -168,39 +230,21 @@ struct vdl2gpu_ctx {
 	bool timing = false;
 	double k_ms[5] = { 0, 0, 0, 0, 0 };                 /* K0, K1, K2a, K2 (+history copy), K3 (+finish) */
 	uint64_t k_launches[5] = { 0, 0, 0, 0, 0 };
-	vdl2_block_trace *d_block_trace = nullptr;          /* VDL2GPU_BLOCK_TRACE=1: per-block scheduling records of K1 / K2 */
+	dev_mem<vdl2_block_trace> d_block_trace;            /* VDL2GPU_BLOCK_TRACE=1: per-block scheduling records of K1 / K2 */
 	uint32_t block_trace_cap = 0;
 	uint32_t graph_nominal = 0;                         /* chunk shape (n_pairs) the graphs are kept for */
-	cudaEvent_t ev_t0 = nullptr;                        /* origin of the timeline (recorded by vdl2gpu_enable_timing) */
+	event_h ev_t0;                                      /* origin of the timeline (recorded by vdl2gpu_enable_timing) */
 	std::vector<float> timeline;                        /* 8 floats per timed chunk: chunk number, then the 7 stage boundaries in ms since ev_t0 */
 	vdl2gpu_stats stats;
 	std::vector<pending_frame> pending;
 	std::vector<std::vector<uint8_t>> blobs;
-	cudaEvent_t ev_drain = nullptr;
-	/* pushed input (ragged contexts, allocated by the first vdl2gpu_push): the receivers' rings (vdl2_push_ring_layout) in
-	 * device memory and their pinned host mirror, the copy stream every push issues its copies on, the event a restart
-	 * records there when it drops queued bytes, and per receiver its queue state */
+	event_h ev_drain;
+	/* pushed input: the rings are push_rings; here the copy stream every push issues its copies on, the event a restart
+	 * records there when it drops queued bytes, and whether the rings exist */
 	std::mutex push_alloc;
 	std::atomic<bool> push_ready{false};
-	uint8_t *d_rings = nullptr, *h_rings = nullptr;
-	std::vector<vdl2_rx_ring> rings;
-	vdl2_rx_ring *d_ring_tab = nullptr;
-	cudaStream_t s_copy = nullptr;
-	cudaEvent_t ev_copied = nullptr, ev_dropped = nullptr;
-	std::vector<std::unique_ptr<push_rx>> push;
-	/* input levels (VDL2GPU_FLAG_INPUT_LEVELS; NULL otherwise): one accumulator per input (stream or receiver), which the
-	 * levels form of K0 adds every converted sample to */
-	vdl2_levels *d_levels = nullptr;
-	/* channel levels (VDL2GPU_FLAG_CHANNEL_LEVELS; NULL otherwise): the per-slot planes the levels form of K2a adds every
-	 * decimated sample to, uint64 [VDL2_CHLV_ROWS][n_chp] then the uint32 peak plane [n_chp] */
-	uint64_t *d_chlv = nullptr;
-	/* spectrum (VDL2GPU_FLAG_SPECTRUM; NULL / empty otherwise): per input its accumulators and waiting samples, the window and
-	 * twiddle tables, and per input its position on its segment grid (samples since the grid's origin: create, joining,
-	 * restart); inputs whose figures a restart zeroes at the start of the next span */
-	vdl2_spec_acc *d_spec = nullptr;
-	vdl2_spec_tab *d_spec_tab = nullptr;
-	std::vector<uint64_t> spec_pos;
-	std::vector<uint32_t> spec_zero;
+	stream_h s_copy;
+	event_h ev_copied, ev_dropped;
 };
 
 static void initial_state(const vdl2gpu_config &cfg, const uint32_t *freqs, const uint32_t *centres, const uint32_t *rates, uint32_t n_ch,
@@ -233,92 +277,33 @@ extern "C" const char *vdl2gpu_strerror(int code) {
 	}
 }
 
-/* the device buffers and chunk slots of setup_layout (nothing may be running on them) */
-static void free_layout(vdl2gpu_ctx *c) {
-	for(auto &s : c->chunks) {
-		if(s.h_raw) cudaFreeHost(s.h_raw);
-		if(s.d_raw) cudaFree(s.d_raw);
-		if(s.h_out) cudaFreeHost(s.h_out);
-		if(s.done) cudaEventDestroy(s.done);
-		if(s.k0_done) cudaEventDestroy(s.k0_done);
-		for(auto &e : s.tk) if(e) cudaEventDestroy(e);
-		for(int i = 0; i < 6; i++) {
-			if(s.g_front[i]) cudaGraphExecDestroy(s.g_front[i]);
-			if(s.g_k2a[i]) cudaGraphExecDestroy(s.g_k2a[i]);
-			if(s.g_back[i]) cudaGraphExecDestroy(s.g_back[i]);
-		}
-		if(s.h_args) cudaFreeHost(s.h_args);
-		if(s.d_args) cudaFree(s.d_args);
-		if(s.h_span) cudaFreeHost(s.h_span);
-		if(s.d_span) cudaFree(s.d_span);
-		if(s.h_restart) cudaFreeHost(s.h_restart);
-		if(s.d_restart) cudaFree(s.d_restart);
-		if(s.h_spec) cudaFreeHost(s.h_spec);
-		if(s.d_spec) cudaFree(s.d_spec);
-	}
-	c->chunks.clear();
-	cudaFree(c->d_samples);
-	for(int i = 0; i < 3; i++) cudaFree(c->d_dec3[i]);
-	for(int i = 0; i < 2; i++) { cudaFree(c->d_phase2[i]); cudaFree(c->d_mag2[i]); }
-	cudaFree(c->d_k1); cudaFree(c->d_k2);
-	cudaFree(c->d_counters); cudaFree(c->d_ready); cudaFree(c->d_ring); cudaFree(c->d_pool); cudaFree(c->d_free); cudaFree(c->d_ctl);
-	cudaFree(c->d_slot_rx); cudaFree(c->d_block_rx);
-	cudaFree(c->d_rx_in); cudaFree(c->d_slot_cls);
-	cudaFree(c->d_levels); cudaFree(c->d_chlv);
-	cudaFree(c->d_spec); cudaFree(c->d_spec_tab);
-}
-
-/* the pushed-input rings and their queues (no push, copy or span may be running on them) */
-static void free_rings(vdl2gpu_ctx *c) {
-	if(c->s_copy) cudaStreamSynchronize(c->s_copy);
-	cudaFree(c->d_rings); cudaFree(c->d_ring_tab);
-	if(c->h_rings) cudaFreeHost(c->h_rings);
-	c->d_rings = c->h_rings = nullptr; c->d_ring_tab = nullptr;
-	c->rings.clear();
-	c->push.clear();
-	c->push_ready = false;
-}
-
 static int free_ctx(vdl2gpu_ctx *c) {
 	if(!c) return VDL2GPU_OK;
 	cudaSetDevice(c->device);
+	/* nothing runs once every stream is idle: the handles may then go in any order */
 	if(c->stream) cudaStreamSynchronize(c->stream);
 	if(c->s_mid) cudaStreamSynchronize(c->s_mid);
 	if(c->s_back) cudaStreamSynchronize(c->s_back);
-	free_rings(c);
-	if(c->ev_copied) cudaEventDestroy(c->ev_copied);
-	if(c->ev_dropped) cudaEventDestroy(c->ev_dropped);
-	if(c->s_copy) cudaStreamDestroy(c->s_copy);
-	free_layout(c);
-	cudaFree(c->d_tab); cudaFree(c->d_events); cudaFree(c->d_block_trace);
-	if(c->ev_input_ready) cudaEventDestroy(c->ev_input_ready);
-	if(c->ev_input_consumed) cudaEventDestroy(c->ev_input_consumed);
-	if(c->ev_drain) cudaEventDestroy(c->ev_drain);
-	if(c->ev_t0) cudaEventDestroy(c->ev_t0);
-	for(int i = 0; i < 2; i++) if(c->ev_k2a_done[i]) cudaEventDestroy(c->ev_k2a_done[i]);
-	for(int i = 0; i < 3; i++) { if(c->ev_k1_done[i]) cudaEventDestroy(c->ev_k1_done[i]); if(c->ev_back_done[i]) cudaEventDestroy(c->ev_back_done[i]); }
-	if(c->s_mid && c->s_mid != c->stream && c->s_mid != c->s_back) cudaStreamDestroy(c->s_mid);
-	if(c->s_back && c->s_back != c->stream) cudaStreamDestroy(c->s_back);
-	if(c->stream) cudaStreamDestroy(c->stream);
+	if(c->s_copy) cudaStreamSynchronize(c->s_copy);
 	delete c;
 	return VDL2GPU_OK;
 }
 
 /* The part of a context that follows from its channels and receivers: the channel slot mapping, span and chunk sizes,
  * burst-pool size, output capacity, receiver tables, per-receiver host records, and every device buffer and chunk slot
- * sized by them.  Create and vdl2gpu_update_receivers both build it here, so the two cannot drift apart.  The checks come
- * first: an EINVAL or ETOOBIG return has touched no device.  The contents of the state planes, the free list and the queue
- * control block are left to the caller.  c->cfg carries the context's flags, max_chunk_bytes and n_inflight; cfg the
- * channels (and, for create, the n_streams the caller asked for); rx / n_rx / rx_ex as for create_impl.  The pool holds at
- * least min_slots slots. */
-static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu_receiver *rx, uint32_t n_rx,
-		const vdl2gpu_receiver_ex *rx_ex, uint32_t min_slots, const char *what) {
-	c->freqs.assign(cfg->freqs, cfg->freqs + cfg->n_channels);
-	c->cfg.freqs = c->freqs.data();
-	c->cfg.n_channels = cfg->n_channels;
-	c->n_ch = cfg->n_channels;
-	c->n_chp = (c->n_ch + 31u) & ~31u;
-	c->lanes = 32; c->full_warps = 0xFFFFFFFFu;
+ * sized by them, built into the empty layout L.  Create and vdl2gpu_update_receivers both build it here, so the two cannot
+ * drift apart.  The checks come first: an EINVAL or ETOOBIG return has touched no device.  The contents of the state
+ * planes, the free list and the queue control block are left to the caller.  cfg: the channels, the inputs (n_streams,
+ * resolved as in create_impl), the flags, max_chunk_bytes and n_inflight with create's defaults, and for a single-rate
+ * context its sample format and oversample factor; rx / n_rx / rx_ex and the context kind as for create_impl; n_sms: the
+ * device's SMs.  The pool holds at least min_slots slots. */
+static int setup_layout(ctx_layout &L, const vdl2gpu_config &cfg, const vdl2gpu_receiver *rx, uint32_t n_rx,
+		const vdl2gpu_receiver_ex *rx_ex, bool receivers, bool mixed, bool ragged, bool lane_streams, int n_sms,
+		uint32_t min_slots, const char *what) {
+	L.freqs.assign(cfg.freqs, cfg.freqs + cfg.n_channels);
+	L.n_ch = cfg.n_channels;
+	L.n_chp = (L.n_ch + 31u) & ~31u;
+	L.n_streams = cfg.n_streams;
 	/* Slot mapping.  K1 and K2 run four-warp blocks, one warp per SM sub-partition, and a chunk's K2 overlaps the next
 	 * chunk's K1.  The block scheduler places a new block on the SM with the most free resources: when a grid leaves SMs
 	 * empty (128 blocks on 132 SMs at 16384 channels), the OTHER kernel's blocks pile up on those SMs two and three deep
@@ -327,194 +312,169 @@ static int setup_layout(vdl2gpu_ctx *c, const vdl2gpu_config *cfg, const vdl2gpu
 	 * sub-partitions, they are dealt out evenly over ALL of them: every warp holds floor or ceil of n_ch / (4 x SMs)
 	 * channels instead of 32 (31 or 32 at 16384 channels on 132 SMs), each of the two kernels launches exactly one block
 	 * per SM, every block lives for the whole kernel, and every SM looks the same to the scheduler. */
-	if(c->receivers || cfg->n_streams <= 1 || cfg->n_streams == cfg->n_channels) {
-		const uint32_t warps_all = 4u * (uint32_t)c->n_sms;
-		if(c->n_ch > 16u * warps_all && c->n_ch <= 32u * warps_all) {
+	if(receivers || cfg.n_streams <= 1 || cfg.n_streams == cfg.n_channels) {
+		const uint32_t warps_all = 4u * (uint32_t)n_sms;
+		if(L.n_ch > 16u * warps_all && L.n_ch <= 32u * warps_all) {
 			const char *e = getenv("VDL2GPU_BALANCE");
 			if(!e || atoi(e)) {
-				c->lanes = (c->n_ch + warps_all - 1u) / warps_all;
-				c->full_warps = c->n_ch - (c->lanes - 1u) * warps_all;       /* warps with `lanes` channels; the rest have lanes - 1 */
-				c->n_chp = warps_all * 32u;
+				L.lanes = (L.n_ch + warps_all - 1u) / warps_all;
+				L.full_warps = L.n_ch - (L.lanes - 1u) * warps_all;       /* warps with `lanes` channels; the rest have lanes - 1 */
+				L.n_chp = warps_all * 32u;
 			}
 		}
 	}
-	const uint32_t max_bytes = c->cfg.max_chunk_bytes;
-	if(c->mixed) {
+	const uint32_t max_bytes = cfg.max_chunk_bytes;
+	if(mixed) {
 		/* the largest span: every receiver's buffer within max_chunk_bytes; the plane's row stride holds the longest row */
 		uint32_t bpd_max = 0;
 		for(uint32_t r = 0; r < n_rx; r++) {
 			bpd_max = std::max(bpd_max, rx_ex[r].oversample * (rx_ex[r].sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u));
-			c->rx_os_max = std::max(c->rx_os_max, rx_ex[r].oversample);
+			L.rx_os_max = std::max(L.rx_os_max, rx_ex[r].oversample);
 		}
-		c->max_span = max_bytes / bpd_max;
-		if(c->max_span == 0) {
+		L.max_span = max_bytes / bpd_max;
+		if(L.max_span == 0) {
 			snprintf(g_last_error, sizeof(g_last_error), "%s: max_chunk_bytes (%u) holds less than one decimated sample of a receiver (%u bytes)",
 					what, max_bytes, bpd_max);
 			return VDL2GPU_EINVAL;
 		}
-		c->max_pairs = (c->max_span * c->rx_os_max + 1u) & ~1u;       /* even row stride: every row of the plane starts 16-byte aligned */
-		c->max_dec = c->max_span + 2;
+		L.max_pairs = (L.max_span * L.rx_os_max + 1u) & ~1u;       /* even row stride: every row of the plane starts 16-byte aligned */
+		L.max_dec = L.max_span + 2;
 	} else {
-		c->max_pairs = max_bytes / (cfg->sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
-		if(c->receivers) c->max_pairs = (c->max_pairs + 1u) & ~1u;     /* even row stride: every receiver row of the plane starts 16-byte aligned */
-		c->max_dec = c->max_pairs / cfg->oversample + 2;
+		L.max_pairs = max_bytes / (cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u);
+		if(receivers) L.max_pairs = (L.max_pairs + 1u) & ~1u;     /* even row stride: every receiver row of the plane starts 16-byte aligned */
+		L.max_dec = L.max_pairs / cfg.oversample + 2;
 	}
-	if((uint64_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp >= (1ull << 32)) {
+	if((uint64_t)(L.max_dec + VDL2_SYNC_BUFLEN) * L.n_chp >= (1ull << 32)) {
 		snprintf(g_last_error, sizeof(g_last_error), "%u channels x %u decimated samples per chunk exceed the 32-bit element index of the kernels; "
-				"use a smaller max_chunk_bytes or shard the channels", c->n_ch, c->max_dec);
+				"use a smaller max_chunk_bytes or shard the channels", L.n_ch, L.max_dec);
 		return VDL2GPU_ETOOBIG;
 	}
-	c->n_slots = std::max(std::max(256u, 3u * c->n_ch), min_slots);
-	c->out_cap = std::max(4u << 20, c->n_ch * 512u);
+	L.n_slots = std::max(std::max(256u, 3u * L.n_ch), min_slots);
+	L.out_cap = std::max(4u << 20, L.n_ch * 512u);
 
 	/* receiver tables (host side) */
 	std::vector<uint32_t> slot_rx, block_rx;
 	std::vector<uint8_t> slot_cls;
-	if(c->receivers) {
+	if(receivers) {
 		/* the slot -> receiver tables K1 stages by */
 		std::vector<uint32_t> rx_first(n_rx + 1, 0);
 		for(uint32_t r = 0; r < n_rx; r++) rx_first[r + 1] = rx_first[r] + rx[r].n_channels;
-		const uint32_t n_blocks = (c->n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
+		const uint32_t n_blocks = (L.n_chp + VDL2_RX_K1_BLOCK - 1) / VDL2_RX_K1_BLOCK;
 		slot_rx.resize((size_t)n_blocks * VDL2_RX_K1_BLOCK); block_rx.resize(2 * (size_t)n_blocks);
-		c->rx_max = vdl2_rx_layout(n_blocks, c->lanes, c->full_warps, c->n_ch, rx_first.data(), n_rx, slot_rx.data(), block_rx.data());
-		c->rx_tile = c->mixed ? vdl2_rx_mixed_tile_groups(c->rx_max, c->rx_os_max) : vdl2_rx_tile_samples(c->rx_max, cfg->oversample);
-		if(c->mixed) {
+		L.rx_max = vdl2_rx_layout(n_blocks, L.lanes, L.full_warps, L.n_ch, rx_first.data(), n_rx, slot_rx.data(), block_rx.data());
+		L.rx_tile = mixed ? vdl2_rx_mixed_tile_groups(L.rx_max, L.rx_os_max) : vdl2_rx_tile_samples(L.rx_max, cfg.oversample);
+		if(mixed) {
 			/* per receiver: oversample, format, place in a span; per slot: rate class; per class: the filter taps of
 			 * input_lpf_init(105000 x os) (src/demod.c:367-370) */
 			std::vector<uint32_t> os(n_rx), fmt(n_rx);
 			for(uint32_t r = 0; r < n_rx; r++) { os[r] = rx_ex[r].oversample; fmt[r] = rx_ex[r].sample_fmt; }
-			c->rx_in.resize(n_rx);
-			c->span_bytes_per_dec = vdl2_rx_span_layout(os.data(), fmt.data(), n_rx, c->rx_in.data());
+			L.rx_in.resize(n_rx);
+			L.span_bytes_per_dec = vdl2_rx_span_layout(os.data(), fmt.data(), n_rx, L.rx_in.data());
 			for(uint32_t r = 0; r < n_rx; r++) {
-				c->span_pairs_per_dec += os[r];
-				c->cls_mask |= 1u << vdl2_rx_class(os[r]);
+				L.span_pairs_per_dec += os[r];
+				L.cls_mask |= 1u << vdl2_rx_class(os[r]);
 			}
 			static const uint32_t class_os[3] = { 10, 13, 20 };
 			for(int k = 0; k < 3; k++) {
 				float A[3], B[3];
 				make_lpf((uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * class_os[k], A, B);
-				c->cls_taps[k][0] = A[0]; c->cls_taps[k][1] = A[1]; c->cls_taps[k][2] = A[2]; c->cls_taps[k][3] = B[1]; c->cls_taps[k][4] = B[2];
+				L.cls_taps[k][0] = A[0]; L.cls_taps[k][1] = A[1]; L.cls_taps[k][2] = A[2]; L.cls_taps[k][3] = B[1]; L.cls_taps[k][4] = B[2];
 			}
 			slot_cls.resize(slot_rx.size());
 			for(size_t s = 0; s < slot_rx.size(); s++) slot_cls[s] = (uint8_t)vdl2_rx_class(os[slot_rx[s]]);
 		}
-		if(c->ragged) {
-			c->rx_pos.assign(n_rx, 0);
-			c->rx_prev.assign(n_rx, 0);
-			c->ch_rx.resize(c->n_ch);
-			for(uint32_t r = 0; r < n_rx; r++) std::fill(c->ch_rx.begin() + rx_first[r], c->ch_rx.begin() + rx_first[r + 1], r);
-			c->rx_first = rx_first;
-			c->rx_centre.resize(n_rx);
-			for(uint32_t r = 0; r < n_rx; r++) c->rx_centre[r] = rx[r].centerfreq;
-			c->rx_restart_pending.assign(n_rx, 0);
-			c->n_restart_pending = 0;
+		if(ragged) {
+			L.rx_pos.assign(n_rx, 0);
+			L.rx_prev.assign(n_rx, 0);
+			L.ch_rx.resize(L.n_ch);
+			for(uint32_t r = 0; r < n_rx; r++) std::fill(L.ch_rx.begin() + rx_first[r], L.ch_rx.begin() + rx_first[r + 1], r);
+			L.rx_first = rx_first;
+			L.rx_centre.resize(n_rx);
+			for(uint32_t r = 0; r < n_rx; r++) L.rx_centre[r] = rx[r].centerfreq;
+			L.rx_restart_pending.assign(n_rx, 0);
+			L.n_restart_pending = 0;
 		}
 	}
 
 	/* device buffers */
-	if(c->lane_streams) CU(cudaMalloc(&c->d_samples, (size_t)c->max_pairs * c->n_chp * sizeof(float2)));
-	else CU(cudaMalloc(&c->d_samples, (size_t)c->n_streams * c->max_pairs * sizeof(float2)));
+	if(lane_streams) CU(cudaMalloc(L.d_samples.put(), (size_t)L.max_pairs * L.n_chp * sizeof(float2)));
+	else CU(cudaMalloc(L.d_samples.put(), (size_t)L.n_streams * L.max_pairs * sizeof(float2)));
 	for(int i = 0; i < 3; i++) {
-		CU(cudaMalloc(&c->d_dec3[i], (size_t)c->max_dec * c->n_chp * sizeof(float2)));
-		CU(cudaMemset(c->d_dec3[i], 0, (size_t)c->max_dec * c->n_chp * sizeof(float2)));
+		CU(cudaMalloc(L.d_dec3[i].put(), (size_t)L.max_dec * L.n_chp * sizeof(float2)));
+		CU(cudaMemset(L.d_dec3[i], 0, (size_t)L.max_dec * L.n_chp * sizeof(float2)));
 	}
 	for(int i = 0; i < 2; i++) {
-		CU(cudaMalloc(&c->d_phase2[i], (size_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp * sizeof(float)));
-		CU(cudaMemset(c->d_phase2[i], 0, (size_t)(c->max_dec + VDL2_SYNC_BUFLEN) * c->n_chp * sizeof(float)));
-		CU(cudaMalloc(&c->d_mag2[i], (size_t)c->max_dec * c->n_chp * sizeof(float)));
+		CU(cudaMalloc(L.d_phase2[i].put(), (size_t)(L.max_dec + VDL2_SYNC_BUFLEN) * L.n_chp * sizeof(float)));
+		CU(cudaMemset(L.d_phase2[i], 0, (size_t)(L.max_dec + VDL2_SYNC_BUFLEN) * L.n_chp * sizeof(float)));
+		CU(cudaMalloc(L.d_mag2[i].put(), (size_t)L.max_dec * L.n_chp * sizeof(float)));
 	}
-	CU(cudaMalloc(&c->d_k1, (size_t)K1_NFIELDS * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_k2, (size_t)K2_NFIELDS * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_counters, (size_t)VDL2_NUM_COUNTERS * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_ring, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
-	CU(cudaMalloc(&c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
-	CU(cudaMalloc(&c->d_free, (size_t)c->n_slots * 4));
-	CU(cudaMalloc(&c->d_ready, (size_t)c->n_slots * 4));
-	CU(cudaMalloc(&c->d_ctl, sizeof(vdl2_queue_ctl)));
-	CU(cudaMemset(c->d_counters, 0, (size_t)VDL2_NUM_COUNTERS * c->n_chp * 4));
-	CU(cudaMemset(c->d_ring, 0, (size_t)VDL2_SYNC_BUFLEN * c->n_chp * 4));
-	CU(cudaMemset(c->d_pool, 0, (size_t)c->n_slots * sizeof(vdl2_burst_slot)));
-	if(c->receivers) {
-		CU(cudaMalloc(&c->d_slot_rx, slot_rx.size() * 4));
-		CU(cudaMalloc(&c->d_block_rx, block_rx.size() * 4));
-		CU(cudaMemcpy(c->d_slot_rx, slot_rx.data(), slot_rx.size() * 4, cudaMemcpyHostToDevice));
-		CU(cudaMemcpy(c->d_block_rx, block_rx.data(), block_rx.size() * 4, cudaMemcpyHostToDevice));
+	CU(cudaMalloc(L.d_k1.put(), (size_t)K1_NFIELDS * L.n_chp * 4));
+	CU(cudaMalloc(L.d_k2.put(), (size_t)K2_NFIELDS * L.n_chp * 4));
+	CU(cudaMalloc(L.d_counters.put(), (size_t)VDL2_NUM_COUNTERS * L.n_chp * 4));
+	CU(cudaMalloc(L.d_ring.put(), (size_t)VDL2_SYNC_BUFLEN * L.n_chp * 4));
+	CU(cudaMalloc(L.d_pool.put(), (size_t)L.n_slots * sizeof(vdl2_burst_slot)));
+	CU(cudaMalloc(L.d_free.put(), (size_t)L.n_slots * 4));
+	CU(cudaMalloc(L.d_ready.put(), (size_t)L.n_slots * 4));
+	CU(cudaMalloc(L.d_ctl.put(), sizeof(vdl2_queue_ctl)));
+	CU(cudaMemset(L.d_counters, 0, (size_t)VDL2_NUM_COUNTERS * L.n_chp * 4));
+	CU(cudaMemset(L.d_ring, 0, (size_t)VDL2_SYNC_BUFLEN * L.n_chp * 4));
+	CU(cudaMemset(L.d_pool, 0, (size_t)L.n_slots * sizeof(vdl2_burst_slot)));
+	if(receivers) {
+		CU(cudaMalloc(L.d_slot_rx.put(), slot_rx.size() * 4));
+		CU(cudaMalloc(L.d_block_rx.put(), block_rx.size() * 4));
+		CU(cudaMemcpy(L.d_slot_rx, slot_rx.data(), slot_rx.size() * 4, cudaMemcpyHostToDevice));
+		CU(cudaMemcpy(L.d_block_rx, block_rx.data(), block_rx.size() * 4, cudaMemcpyHostToDevice));
 	}
-	if(c->cfg.flags & VDL2GPU_FLAG_INPUT_LEVELS) {
-		CU(cudaMalloc(&c->d_levels, (size_t)c->n_streams * sizeof(vdl2_levels)));
-		CU(cudaMemset(c->d_levels, 0, (size_t)c->n_streams * sizeof(vdl2_levels)));
+	if(cfg.flags & VDL2GPU_FLAG_INPUT_LEVELS) {
+		CU(cudaMalloc(L.d_levels.put(), (size_t)L.n_streams * sizeof(vdl2_levels)));
+		CU(cudaMemset(L.d_levels, 0, (size_t)L.n_streams * sizeof(vdl2_levels)));
 	}
-	if(c->cfg.flags & VDL2GPU_FLAG_CHANNEL_LEVELS) {
-		const size_t bytes = (size_t)VDL2_CHLV_ROWS * c->n_chp * 8 + (size_t)c->n_chp * 4;
-		CU(cudaMalloc(&c->d_chlv, bytes));
-		CU(cudaMemset(c->d_chlv, 0, bytes));
+	if(cfg.flags & VDL2GPU_FLAG_CHANNEL_LEVELS) {
+		const size_t bytes = (size_t)VDL2_CHLV_ROWS * L.n_chp * 8 + (size_t)L.n_chp * 4;
+		CU(cudaMalloc(L.d_chlv.put(), bytes));
+		CU(cudaMemset(L.d_chlv, 0, bytes));
 	}
-	if(c->cfg.flags & VDL2GPU_FLAG_SPECTRUM) {
-		CU(cudaMalloc(&c->d_spec, (size_t)c->n_streams * sizeof(vdl2_spec_acc)));
-		CU(cudaMemset(c->d_spec, 0, (size_t)c->n_streams * sizeof(vdl2_spec_acc)));
+	if(cfg.flags & VDL2GPU_FLAG_SPECTRUM) {
+		CU(cudaMalloc(L.d_spec.put(), (size_t)L.n_streams * sizeof(vdl2_spec_acc)));
+		CU(cudaMemset(L.d_spec, 0, (size_t)L.n_streams * sizeof(vdl2_spec_acc)));
 		std::unique_ptr<vdl2_spec_tab> tab(new vdl2_spec_tab);
 		vdl2_spec_make_tab(tab.get());
-		CU(cudaMalloc(&c->d_spec_tab, sizeof(vdl2_spec_tab)));
-		CU(cudaMemcpy(c->d_spec_tab, tab.get(), sizeof(vdl2_spec_tab), cudaMemcpyHostToDevice));
-		c->spec_pos.assign(c->n_streams, 0);
-		c->spec_zero.clear();
+		CU(cudaMalloc(L.d_spec_tab.put(), sizeof(vdl2_spec_tab)));
+		CU(cudaMemcpy(L.d_spec_tab, tab.get(), sizeof(vdl2_spec_tab), cudaMemcpyHostToDevice));
+		L.spec_pos.assign(L.n_streams, 0);
+		L.spec_zero.clear();
 	}
-	if(c->mixed) {
-		CU(cudaMalloc(&c->d_rx_in, c->rx_in.size() * sizeof(vdl2_rx_input)));
-		CU(cudaMalloc(&c->d_slot_cls, slot_cls.size()));
-		CU(cudaMemcpy(c->d_rx_in, c->rx_in.data(), c->rx_in.size() * sizeof(vdl2_rx_input), cudaMemcpyHostToDevice));
-		CU(cudaMemcpy(c->d_slot_cls, slot_cls.data(), slot_cls.size(), cudaMemcpyHostToDevice));
+	if(mixed) {
+		CU(cudaMalloc(L.d_rx_in.put(), L.rx_in.size() * sizeof(vdl2_rx_input)));
+		CU(cudaMalloc(L.d_slot_cls.put(), slot_cls.size()));
+		CU(cudaMemcpy(L.d_rx_in, L.rx_in.data(), L.rx_in.size() * sizeof(vdl2_rx_input), cudaMemcpyHostToDevice));
+		CU(cudaMemcpy(L.d_slot_cls, slot_cls.data(), slot_cls.size(), cudaMemcpyHostToDevice));
 	}
 
-	c->chunks.resize(c->cfg.n_inflight);
-	for(auto &s : c->chunks) {
+	L.chunks.resize(cfg.n_inflight);
+	for(auto &s : L.chunks) {
 		/* h_raw / d_raw (max_chunk_bytes x n_streams each) are allocated by the first vdl2gpu_submit: hosts that only
 		 * use vdl2gpu_submit_device never need them */
-		CU(cudaHostAlloc((void **)&s.h_args, sizeof(vdl2_chunk_args), cudaHostAllocDefault));
-		CU(cudaMalloc(&s.d_args, sizeof(vdl2_chunk_args)));
-		if(c->ragged) {
-			CU(cudaHostAlloc((void **)&s.h_span, (size_t)n_rx * sizeof(vdl2_rx_span), cudaHostAllocDefault));
-			CU(cudaMalloc(&s.d_span, (size_t)n_rx * sizeof(vdl2_rx_span)));
-			CU(cudaHostAlloc((void **)&s.h_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart), cudaHostAllocDefault));
-			CU(cudaMalloc(&s.d_restart, (size_t)c->n_chp * sizeof(vdl2_rx_restart)));
-			CU(cudaEventCreateWithFlags(&s.k0_done, cudaEventDisableTiming));
+		CU(cudaHostAlloc((void **)s.h_args.put(), sizeof(vdl2_chunk_args), cudaHostAllocDefault));
+		CU(cudaMalloc(s.d_args.put(), sizeof(vdl2_chunk_args)));
+		if(ragged) {
+			CU(cudaHostAlloc((void **)s.h_span.put(), (size_t)n_rx * sizeof(vdl2_rx_span), cudaHostAllocDefault));
+			CU(cudaMalloc(s.d_span.put(), (size_t)n_rx * sizeof(vdl2_rx_span)));
+			CU(cudaHostAlloc((void **)s.h_restart.put(), (size_t)L.n_chp * sizeof(vdl2_rx_restart), cudaHostAllocDefault));
+			CU(cudaMalloc(s.d_restart.put(), (size_t)L.n_chp * sizeof(vdl2_rx_restart)));
+			CU(cudaEventCreateWithFlags(s.k0_done.put(), cudaEventDisableTiming));
 		}
-		CU(cudaHostAlloc((void **)&s.h_out, sizeof(vdl2_out_header) + c->out_cap, cudaHostAllocMapped));
+		CU(cudaHostAlloc((void **)s.h_out.put(), sizeof(vdl2_out_header) + L.out_cap, cudaHostAllocMapped));
 		CU(cudaHostGetDevicePointer((void **)&s.d_out, s.h_out, 0));
-		if(c->d_spec) {
-			CU(cudaHostAlloc((void **)&s.h_spec, (size_t)c->n_streams * sizeof(vdl2_spec_span), cudaHostAllocDefault));
-			CU(cudaMalloc(&s.d_spec, (size_t)c->n_streams * sizeof(vdl2_spec_span)));
+		if(L.d_spec) {
+			CU(cudaHostAlloc((void **)s.h_spec.put(), (size_t)L.n_streams * sizeof(vdl2_spec_span), cudaHostAllocDefault));
+			CU(cudaMalloc(s.d_spec.put(), (size_t)L.n_streams * sizeof(vdl2_spec_span)));
 		}
 		memset(s.h_out, 0, sizeof(vdl2_out_header));
-		CU(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-		for(auto &ev : s.tk) CU(cudaEventCreate(&ev));
+		CU(cudaEventCreateWithFlags(s.done.put(), cudaEventDisableTiming));
+		for(auto &ev : s.tk) CU(cudaEventCreate(ev.put()));
 	}
 	return VDL2GPU_OK;
-}
-
-/* exchange what setup_layout built (the switch of vdl2gpu_update_receivers) */
-static void swap_layout(vdl2gpu_ctx *a, vdl2gpu_ctx *b) {
-	using std::swap;
-	swap(a->freqs, b->freqs);
-	a->cfg.freqs = a->freqs.data(); b->cfg.freqs = b->freqs.data();
-	swap(a->cfg.n_channels, b->cfg.n_channels); swap(a->cfg.n_streams, b->cfg.n_streams);
-	swap(a->n_ch, b->n_ch); swap(a->n_chp, b->n_chp); swap(a->lanes, b->lanes); swap(a->full_warps, b->full_warps);
-	swap(a->n_streams, b->n_streams);
-	swap(a->max_pairs, b->max_pairs); swap(a->max_dec, b->max_dec); swap(a->max_span, b->max_span);
-	swap(a->n_slots, b->n_slots); swap(a->out_cap, b->out_cap);
-	swap(a->rx_tile, b->rx_tile); swap(a->rx_max, b->rx_max); swap(a->rx_os_max, b->rx_os_max); swap(a->cls_mask, b->cls_mask);
-	swap(a->cls_taps, b->cls_taps);
-	swap(a->rx_in, b->rx_in); swap(a->span_bytes_per_dec, b->span_bytes_per_dec); swap(a->span_pairs_per_dec, b->span_pairs_per_dec);
-	swap(a->rx_pos, b->rx_pos); swap(a->rx_prev, b->rx_prev); swap(a->ch_rx, b->ch_rx);
-	swap(a->rx_centre, b->rx_centre); swap(a->rx_first, b->rx_first);
-	swap(a->rx_restart_pending, b->rx_restart_pending); swap(a->n_restart_pending, b->n_restart_pending);
-	swap(a->d_slot_rx, b->d_slot_rx); swap(a->d_block_rx, b->d_block_rx); swap(a->d_rx_in, b->d_rx_in); swap(a->d_slot_cls, b->d_slot_cls);
-	swap(a->d_samples, b->d_samples); swap(a->d_dec3, b->d_dec3); swap(a->d_phase2, b->d_phase2); swap(a->d_mag2, b->d_mag2);
-	swap(a->d_k1, b->d_k1); swap(a->d_k2, b->d_k2); swap(a->d_counters, b->d_counters); swap(a->d_ring, b->d_ring);
-	swap(a->d_pool, b->d_pool); swap(a->d_free, b->d_free); swap(a->d_ready, b->d_ready); swap(a->d_ctl, b->d_ctl);
-	swap(a->d_levels, b->d_levels); swap(a->d_chlv, b->d_chlv);
-	swap(a->d_spec, b->d_spec); swap(a->d_spec_tab, b->d_spec_tab); swap(a->spec_pos, b->spec_pos); swap(a->spec_zero, b->spec_zero);
-	swap(a->chunks, b->chunks);
 }
 
 /* rx / n_rx: the receivers of a multi-receiver context (vdl2gpu_create_receivers, validated there), NULL / 0 otherwise;
@@ -542,18 +502,18 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	c->receivers = rx != nullptr;
 	c->mixed = rx_ex != nullptr;
 	c->ragged = c->mixed && (cfg->flags & VDL2GPU_FLAG_RAGGED);
-	c->n_streams = c->receivers ? n_rx : cfg->n_streams ? cfg->n_streams : 1u;
-	c->cfg.n_streams = c->n_streams;
-	c->lane_streams = !c->receivers && c->n_streams > 1 && c->n_streams == cfg->n_channels;     /* one stream per channel */
+	const uint32_t n_streams = c->receivers ? n_rx : cfg->n_streams ? cfg->n_streams : 1u;
+	c->cfg.n_streams = n_streams;
+	c->lane_streams = !c->receivers && n_streams > 1 && n_streams == cfg->n_channels;     /* one stream per channel */
 	if(c->lane_streams) {
 		c->ch_per_stream = 1;
-	} else if(c->n_streams > 1 && !c->receivers) {      /* (receivers: any channel count each, see the receiver tables below) */
-		if(cfg->n_channels % c->n_streams != 0 || (cfg->n_channels / c->n_streams) % 32u != 0) {
+	} else if(n_streams > 1 && !c->receivers) {         /* (receivers: any channel count each, see the receiver tables below) */
+		if(cfg->n_channels % n_streams != 0 || (cfg->n_channels / n_streams) % 32u != 0) {
 			snprintf(g_last_error, sizeof(g_last_error), "independent-streams mode needs n_channels = n_streams x C with C = 1 or a multiple of 32 (got %u channels, %u streams)",
-					cfg->n_channels, c->n_streams);
+					cfg->n_channels, n_streams);
 			return VDL2GPU_EINVAL;
 		}
-		c->ch_per_stream = cfg->n_channels / c->n_streams;
+		c->ch_per_stream = cfg->n_channels / n_streams;
 	}
 	{
 		const char *e;
@@ -570,37 +530,42 @@ static int create_impl(const vdl2gpu_config *cfg, vdl2gpu_ctx *c, const vdl2gpu_
 	c->cfg.max_chunk_bytes = cfg->max_chunk_bytes ? cfg->max_chunk_bytes : (1u << 20);
 	c->cfg.n_inflight = cfg->n_inflight ? cfg->n_inflight : 4u;
 	c->event_cap = (cfg->flags & VDL2GPU_FLAG_TRACE) ? (1u << 20) : 1u;
-	int rc = setup_layout(c, cfg, rx, n_rx, rx_ex, 0, c->mixed ? "vdl2gpu_create_mixed_receivers" : c->receivers ? "vdl2gpu_create_receivers" : "vdl2gpu_create");
+	ctx_layout L;
+	int rc = setup_layout(L, c->cfg, rx, n_rx, rx_ex, c->receivers, c->mixed, c->ragged, c->lane_streams, c->n_sms, 0,
+			c->mixed ? "vdl2gpu_create_mixed_receivers" : c->receivers ? "vdl2gpu_create_receivers" : "vdl2gpu_create");
 	if(rc) return rc;
+	static_cast<ctx_layout &>(*c) = std::move(L);
+	c->cfg.freqs = nullptr;                             /* the caller's array: the layout holds a copy */
 	/* (mixed receivers: the rate only enters the filter taps of these tables, which the mixed K1 takes per rate class) */
 	make_tables(c->tab, c->mixed ? (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * c->rx_os_max : cfg->sample_rate);
 	memset(&c->stats, 0, sizeof(c->stats));
 
 	/* equal (default) priorities: raising either stage's priority slowed the pair down (tools/probe_overlap.py) */
-	CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+	CU(cudaStreamCreateWithFlags(c->stream.put(), cudaStreamNonBlocking));
 	if(cfg->flags & VDL2GPU_FLAG_NO_OVERLAP) { c->s_back = c->stream; c->s_mid = c->stream; }
 	else {
-		CU(cudaStreamCreateWithFlags(&c->s_back, cudaStreamNonBlocking));
-		if(c->stages == 3) CU(cudaStreamCreateWithFlags(&c->s_mid, cudaStreamNonBlocking));
-		else c->s_mid = c->s_back;
+		CU(cudaStreamCreateWithFlags(c->back_stream.put(), cudaStreamNonBlocking));
+		c->s_back = c->back_stream;
+		if(c->stages == 3) CU(cudaStreamCreateWithFlags(c->mid_stream.put(), cudaStreamNonBlocking));
+		c->s_mid = c->stages == 3 ? c->mid_stream : c->back_stream;
 	}
-	for(int i = 0; i < 2; i++) CU(cudaEventCreateWithFlags(&c->ev_k2a_done[i], cudaEventDisableTiming));
+	for(int i = 0; i < 2; i++) CU(cudaEventCreateWithFlags(c->ev_k2a_done[i].put(), cudaEventDisableTiming));
 	for(int i = 0; i < 3; i++) {
-		CU(cudaEventCreateWithFlags(&c->ev_k1_done[i], cudaEventDisableTiming));
-		CU(cudaEventCreateWithFlags(&c->ev_back_done[i], cudaEventDisableTiming));
+		CU(cudaEventCreateWithFlags(c->ev_k1_done[i].put(), cudaEventDisableTiming));
+		CU(cudaEventCreateWithFlags(c->ev_back_done[i].put(), cudaEventDisableTiming));
 	}
-	CU(cudaEventCreateWithFlags(&c->ev_input_ready, cudaEventDisableTiming));
-	CU(cudaEventCreateWithFlags(&c->ev_input_consumed, cudaEventDisableTiming));
-	CU(cudaEventCreateWithFlags(&c->ev_drain, cudaEventDisableTiming));
+	CU(cudaEventCreateWithFlags(c->ev_input_ready.put(), cudaEventDisableTiming));
+	CU(cudaEventCreateWithFlags(c->ev_input_consumed.put(), cudaEventDisableTiming));
+	CU(cudaEventCreateWithFlags(c->ev_drain.put(), cudaEventDisableTiming));
 	if(c->block_trace_cap) {
 		const size_t bytes = sizeof(vdl2_block_trace) + (size_t)c->block_trace_cap * sizeof(vdl2_block_rec);
-		CU(cudaMalloc(&c->d_block_trace, bytes));
+		CU(cudaMalloc(c->d_block_trace.put(), bytes));
 		CU(cudaMemset(c->d_block_trace, 0, bytes));
 		CU(cudaMemcpy(&c->d_block_trace->cap, &c->block_trace_cap, 4, cudaMemcpyHostToDevice));
 	}
-	CU(cudaMalloc(&c->d_tab, sizeof(vdl2_tables)));
+	CU(cudaMalloc(c->d_tab.put(), sizeof(vdl2_tables)));
 	CU(cudaMemcpy(c->d_tab, &c->tab.t, sizeof(vdl2_tables), cudaMemcpyHostToDevice));
-	CU(cudaMalloc(&c->d_events, (size_t)c->event_cap * sizeof(vdl2gpu_event)));
+	CU(cudaMalloc(c->d_events.put(), (size_t)c->event_cap * sizeof(vdl2gpu_event)));
 
 	std::vector<uint32_t> k1, k2, centres, rates;
 	if(c->receivers) {
@@ -850,16 +815,17 @@ static void harvest(vdl2gpu_ctx *c, chunk_slot &s) {
 		s.timed = false;
 	}
 	/* one copy out of the mapped region (header + the bytes K3 used), so the region can be handed back to the device at once */
-	const vdl2_out_header *h = reinterpret_cast<const vdl2_out_header *>(s.h_out);
+	const uint8_t *out = s.h_out;
+	const vdl2_out_header *h = reinterpret_cast<const vdl2_out_header *>(out);
 	const uint32_t used = std::min(h->bytes_used, c->out_cap);
-	c->blobs.emplace_back(s.h_out, s.h_out + sizeof(vdl2_out_header) + used);
+	c->blobs.emplace_back(out, out + sizeof(vdl2_out_header) + used);
 	const uint32_t blob_id = (uint32_t)c->blobs.size() - 1;
 	/* decimated samples per second (105000 for every receiver of a mixed context, whose config carries no rate) */
 	const double rate = c->mixed ? (double)VDL2_SYMBOL_RATE * VDL2_SPS : (double)c->cfg.sample_rate / (double)c->cfg.oversample;
 	stamp_fn stamp;
 	if(s.pushed) stamp = [c](uint32_t chan, uint64_t sync, double &ts) { return push_stamp(c, chan, sync, ts); };
 	parse_region(c->blobs.back().data(), c->out_cap, rate, s.arrival, s.dec_base + s.n_dec, blob_id, c->pending, c->stats,
-			c->ragged ? s.h_span : nullptr, c->ch_rx.data(), s.pushed ? &stamp : nullptr);
+			c->ragged ? s.h_span.get() : nullptr, c->ch_rx.data(), s.pushed ? &stamp : nullptr);
 	c->stats.chunks_completed++;
 	s.busy = false;
 }
@@ -896,8 +862,8 @@ static int ensure_raw(vdl2gpu_ctx *c, chunk_slot &s) {
 		snprintf(g_last_error, sizeof(g_last_error), "vdl2gpu_submit: n_streams x max_chunk_bytes must stay below 4 GiB (use vdl2gpu_submit_device)");
 		return VDL2GPU_ETOOBIG;
 	}
-	CU(cudaHostAlloc((void **)&s.h_raw, bytes, cudaHostAllocDefault));
-	CU(cudaMalloc(&s.d_raw, bytes));
+	CU(cudaHostAlloc((void **)s.h_raw.put(), bytes, cudaHostAllocDefault));
+	CU(cudaMalloc(s.d_raw.put(), bytes));
 	return VDL2GPU_OK;
 }
 
@@ -933,7 +899,7 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	memcpy(p1.cls_taps, c->cls_taps, sizeof(p1.cls_taps));
 	/* the default walk (variant 5) computes the four magnitudes a block needs from the staged samples: no magnitude plane */
 	const bool need_mag = (c->k2_variant & 0xFF) >= 0 && (c->k2_variant & 0xFF) <= 4;
-	pa.dec = d_dec; pa.phase = c->d_phase2[pb]; pa.mag = need_mag ? c->d_mag2[pb] : nullptr; pa.phase_prev = c->d_phase2[pb ^ 1];
+	pa.dec = d_dec; pa.phase = c->d_phase2[pb]; pa.mag = need_mag ? c->d_mag2[pb].get() : nullptr; pa.phase_prev = c->d_phase2[pb ^ 1];
 	pa.n_dec = n_dec; pa.prev_n_dec = prev_n_dec; pa.n_ch = c->n_ch; pa.n_chp = c->n_chp; pa.lanes = c->lanes; pa.full_warps = c->full_warps;
 	pa.mode = (uint32_t)c->k2a_mode; pa.split = c->k2a_split; pa.ca = ca; pa.chlv = c->d_chlv;
 	p2.dec = d_dec; p2.phase = c->d_phase2[pb]; p2.mag = c->d_mag2[pb]; p2.hist_tmp = nullptr; p2.n_dec = n_dec; p2.n_ch = c->n_ch; p2.n_chp = c->n_chp;
@@ -944,7 +910,7 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
 	p2.variant = (uint32_t)c->k2_variant; p2.k2a_mode = (uint32_t)c->k2a_mode; p2.ca = ca;
 	p1.rx_span = s.d_span; pa.slot_rx = c->d_slot_rx; pa.rx_span = s.d_span; p2.slot_rx = c->d_slot_rx; p2.rx_span = s.d_span;   /* (NULL unless ragged) */
 	/* the restart table only on a span that restarts receivers, which is never captured (NULL in every graph) */
-	const vdl2_rx_restart *rs = (s.restart && !ca) ? s.d_restart : nullptr;
+	const vdl2_rx_restart *rs = (s.restart && !ca) ? s.d_restart.get() : nullptr;
 	p1.rx_restart = rs; pa.rx_restart = rs; p2.rx_restart = rs;
 	p3.pool = c->d_pool; p3.free_list = c->d_free; p3.ready = c->d_ready; p3.ctl = c->d_ctl; p3.tables = c->d_tab;
 	p3.out = s.d_out; p3.out_cap = c->out_cap; p3.n_chp = c->n_chp; p3.counters = c->d_counters; p3.abandoned = rs ? 1u : 0u;
@@ -957,13 +923,13 @@ static void fill_params(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_
  * launches.  Everything that differs between two chunks of the same shape (input pointer, decimation phase, sample
  * counts, absolute sample index) travels in the chunk-argument block the front graph copies to the device first. */
 template<typename F>
-static int capture_one(cudaStream_t st, cudaGraphExec_t *out, F body) {
+static int capture_one(cudaStream_t st, graph_exec_h &out, F body) {
 	cudaGraph_t g = nullptr;
 	CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed));
 	int rc = body();
 	cudaError_t e = cudaStreamEndCapture(st, &g);
 	if(rc != 0 || e != cudaSuccess) { if(g) cudaGraphDestroy(g); cudaGetLastError(); return rc ? rc : fail_cuda(e, "cudaStreamEndCapture", __LINE__); }
-	e = cudaGraphInstantiate(out, g, 0);
+	e = cudaGraphInstantiate(out.put(), g, 0);
 	cudaGraphDestroy(g);
 	if(e != cudaSuccess) return fail_cuda(e, "cudaGraphInstantiate", __LINE__);
 	return VDL2GPU_OK;
@@ -976,10 +942,10 @@ static inline uint32_t chain_os(const vdl2gpu_ctx *c) { return c->mixed ? 1u : c
  * counts, and pushed spans, which read the receivers' rings), one column per stream (one stream per channel) or one row
  * per stream.  n_pairs: samples per stream, or the span's decimated samples (its width when ragged).  ca: graph capture. */
 static int launch_k0(vdl2gpu_ctx *c, const chunk_slot &s, const void *raw, uint32_t n_pairs, uint32_t fmt, const vdl2_chunk_args *ca) {
-	float *out = reinterpret_cast<float *>(c->d_samples);
+	float *out = reinterpret_cast<float *>(c->d_samples.get());
 	const uint32_t bpp = c->cfg.sample_fmt == VDL2GPU_FMT_S16_LE ? 4u : 2u;
 	if(c->mixed) {
-		const vdl2_k0_rows rows = { s.pushed ? c->d_rings : raw, c->d_rx_in, s.d_span, s.pushed ? c->d_ring_tab : nullptr };
+		const vdl2_k0_rows rows = { s.pushed ? c->d_rings : raw, c->d_rx_in, s.d_span, s.pushed ? c->d_ring_tab.get() : nullptr };
 		KL(vdl2_launch_k0_rows(&rows, n_pairs, c->n_streams, c->rx_os_max, c->d_tab->levels, out, c->max_pairs, ca, c->d_levels, c->stream));
 	} else if(c->lane_streams) KL(vdl2_launch_k0_lanes(raw, n_pairs, fmt, c->d_tab->levels, out, c->n_streams, n_pairs * bpp, c->n_chp,
 			c->lanes, c->full_warps, ca, c->d_levels, c->stream));
@@ -992,7 +958,7 @@ static int launch_k0(vdl2gpu_ctx *c, const chunk_slot &s, const void *raw, uint3
  * and before K2a, so the lock step of K2 and K1 launched together into an empty machine after K2a is left as it was. */
 static int launch_spectrum(vdl2gpu_ctx *c, chunk_slot &s, uint32_t n_pairs) {
 	CU(cudaMemcpyAsync(s.d_spec, s.h_spec, c->n_streams * sizeof(vdl2_spec_span), cudaMemcpyHostToDevice, c->stream));
-	KL(vdl2_launch_spectrum(reinterpret_cast<const float *>(c->d_samples), c->mixed ? n_pairs * c->rx_os_max : n_pairs, c->n_streams,
+	KL(vdl2_launch_spectrum(reinterpret_cast<const float *>(c->d_samples.get()), c->mixed ? n_pairs * c->rx_os_max : n_pairs, c->n_streams,
 			c->lane_streams ? c->n_chp : c->max_pairs, c->lane_streams ? c->lanes : 0u, c->full_warps, s.d_spec, c->d_spec_tab, c->d_spec,
 			c->stream));
 	return VDL2GPU_OK;
@@ -1046,15 +1012,13 @@ static int launch_back(vdl2gpu_ctx *c, const vdl2_k2_params &p2, const vdl2_k3_p
 static int ensure_graphs(vdl2gpu_ctx *c, chunk_slot &s, uint64_t seq, uint32_t n_pairs, uint32_t k0_fmt) {
 	const int k = (int)(seq % 6u);
 	if(s.g_front[k] && s.graph_pairs[k] == n_pairs) return VDL2GPU_OK;
-	if(s.g_front[k]) { cudaGraphExecDestroy(s.g_front[k]); s.g_front[k] = nullptr; }
-	if(s.g_k2a[k]) { cudaGraphExecDestroy(s.g_k2a[k]); s.g_k2a[k] = nullptr; }
-	if(s.g_back[k]) { cudaGraphExecDestroy(s.g_back[k]); s.g_back[k] = nullptr; }
+	s.g_front[k].reset(); s.g_k2a[k].reset(); s.g_back[k].reset();
 	vdl2_k1_params p1; vdl2_k2a_params pa; vdl2_k2_params p2; vdl2_k3_params p3;
 	const uint32_t os = chain_os(c);
 	fill_params(c, s, seq, n_pairs, 0, (os - 1 + n_pairs) / os, 0, 0, s.d_args, p1, pa, p2, p3);
-	int rc = capture_one(c->stream, &s.g_front[k], [&] { return launch_front(c, s, nullptr, n_pairs, k0_fmt, p1, s.d_args); });
-	if(rc == 0) rc = capture_one(c->s_mid, &s.g_k2a[k], [&] { KL(vdl2_launch_k2a_warps(&pa, c->s_mid)); return 0; });
-	if(rc == 0) rc = capture_one(c->s_back, &s.g_back[k], [&] { return launch_back(c, p2, p3, nullptr); });
+	int rc = capture_one(c->stream, s.g_front[k], [&] { return launch_front(c, s, nullptr, n_pairs, k0_fmt, p1, s.d_args); });
+	if(rc == 0) rc = capture_one(c->s_mid, s.g_k2a[k], [&] { KL(vdl2_launch_k2a_warps(&pa, c->s_mid)); return 0; });
+	if(rc == 0) rc = capture_one(c->s_back, s.g_back[k], [&] { return launch_back(c, p2, p3, nullptr); });
 	if(rc == 0) s.graph_pairs[k] = n_pairs;
 	return rc;
 }
@@ -1121,7 +1085,7 @@ static int run_chain(vdl2gpu_ctx *c, chunk_slot &s, const void *d_raw, uint32_t 
 		if(s.timed) CU(cudaEventRecord(s.tk[4], c->s_back));
 		c->stats.graph_launches += 3;
 	} else {
-		int rc = launch_back(c, p2, p3, s.timed ? s.tk[4] : nullptr);
+		int rc = launch_back(c, p2, p3, s.timed ? s.tk[4].get() : nullptr);
 		if(rc) return rc;
 	}
 	if(s.timed) CU(cudaEventRecord(s.tk[5], c->s_back));
@@ -1365,35 +1329,30 @@ extern "C" int vdl2gpu_submit_ragged_device(vdl2gpu_ctx *c, const void *dev_iq, 
 /* ------------------------------------------------------------------------------------------------
  * pushed input (vdl2gpu_push, vdl2gpu_submit_pushed; see DESIGN.md, "Pushed input", for the ordering rules)
  * ---------------------------------------------------------------------------------------------- */
-/* the rings of the current receiver list, their pinned host mirror and empty queues; on failure nothing stays allocated */
-static int alloc_rings_impl(vdl2gpu_ctx *c) {
-	const uint32_t n_rx = c->n_streams;
-	c->rings.resize(n_rx);
-	const uint64_t total = vdl2_push_ring_layout(c->rx_in.data(), n_rx, c->cfg.max_chunk_bytes, c->max_span, c->rings.data());
-	CU(cudaMalloc(&c->d_rings, total));
-	CU(cudaHostAlloc((void **)&c->h_rings, total, cudaHostAllocDefault));
-	CU(cudaMalloc(&c->d_ring_tab, (size_t)n_rx * sizeof(vdl2_rx_ring)));
-	CU(cudaMemcpy(c->d_ring_tab, c->rings.data(), (size_t)n_rx * sizeof(vdl2_rx_ring), cudaMemcpyHostToDevice));
-	c->push.resize(n_rx);
-	for(auto &q : c->push) q.reset(new push_rx());
+/* the rings of layout L's receivers, their pinned host mirror and empty queues, built into the empty P (on failure P holds
+ * what it got, and frees it) */
+static int alloc_rings(push_rings &P, const ctx_layout &L, uint32_t max_chunk_bytes) {
+	const uint32_t n_rx = L.n_streams;
+	P.rings.resize(n_rx);
+	const uint64_t total = vdl2_push_ring_layout(L.rx_in.data(), n_rx, max_chunk_bytes, L.max_span, P.rings.data());
+	CU(cudaMalloc(P.d_rings.put(), total));
+	CU(cudaHostAlloc((void **)P.h_rings.put(), total, cudaHostAllocDefault));
+	CU(cudaMalloc(P.d_ring_tab.put(), (size_t)n_rx * sizeof(vdl2_rx_ring)));
+	CU(cudaMemcpy(P.d_ring_tab, P.rings.data(), (size_t)n_rx * sizeof(vdl2_rx_ring), cudaMemcpyHostToDevice));
+	P.push.resize(n_rx);
+	for(auto &q : P.push) q.reset(new push_rx());
 	return VDL2GPU_OK;
 }
 
-static int alloc_rings(vdl2gpu_ctx *c) {
-	const int rc = alloc_rings_impl(c);
-	if(rc) free_rings(c);
-	return rc;
-}
-
 /* len bytes at stream position pos of receiver r's ring: into the host mirror, then one copy per piece on stream st */
-static int ring_write(vdl2gpu_ctx *c, cudaStream_t st, uint32_t r, uint64_t pos, const uint8_t *src, uint32_t len) {
-	const vdl2_rx_ring &rg = c->rings[r];
+static int ring_write(const push_rings &P, cudaStream_t st, uint32_t r, uint64_t pos, const uint8_t *src, uint32_t len) {
+	const vdl2_rx_ring &rg = P.rings[r];
 	const vdl2_ring_segs sg = vdl2_ring_segments(rg.cap, pos, len);
 	for(int k = 0; k < 2; k++) {
 		if(!sg.len[k]) continue;
-		uint8_t *h = c->h_rings + rg.base + sg.off[k];
+		uint8_t *h = P.h_rings + rg.base + sg.off[k];
 		memcpy(h, src, sg.len[k]);
-		CU(cudaMemcpyAsync(c->d_rings + rg.base + sg.off[k], h, sg.len[k], cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(P.d_rings + rg.base + sg.off[k], h, sg.len[k], cudaMemcpyHostToDevice, st));
 		src += sg.len[k];
 	}
 	return VDL2GPU_OK;
@@ -1421,12 +1380,14 @@ extern "C" int vdl2gpu_push(vdl2gpu_ctx *c, uint32_t r, const void *iq, uint32_t
 		std::lock_guard<std::mutex> lk(c->push_alloc);
 		if(!c->push_ready) {
 			if(!c->s_copy) {
-				CU(cudaStreamCreateWithFlags(&c->s_copy, cudaStreamNonBlocking));
-				CU(cudaEventCreateWithFlags(&c->ev_copied, cudaEventDisableTiming));
-				CU(cudaEventCreateWithFlags(&c->ev_dropped, cudaEventDisableTiming));
+				CU(cudaStreamCreateWithFlags(c->s_copy.put(), cudaStreamNonBlocking));
+				CU(cudaEventCreateWithFlags(c->ev_copied.put(), cudaEventDisableTiming));
+				CU(cudaEventCreateWithFlags(c->ev_dropped.put(), cudaEventDisableTiming));
 			}
-			const int rc = alloc_rings(c);
+			push_rings P;
+			const int rc = alloc_rings(P, *c, c->cfg.max_chunk_bytes);
 			if(rc) return rc;
+			static_cast<push_rings &>(*c) = std::move(P);
 			c->push_ready = true;
 		}
 	}
@@ -1454,7 +1415,7 @@ extern "C" int vdl2gpu_push(vdl2gpu_ctx *c, uint32_t r, const void *iq, uint32_t
 			q.room.wait(lk);
 		}
 	}
-	const int rc = ring_write(c, c->s_copy, r, q.head, static_cast<const uint8_t *>(iq), len);
+	const int rc = ring_write(*c, c->s_copy, r, q.head, static_cast<const uint8_t *>(iq), len);
 	if(rc) return rc;
 	/* published only now: the copies are issued, so an event submit_pushed records on the copy stream after reading head
 	 * covers every byte before it */
@@ -1463,35 +1424,26 @@ extern "C" int vdl2gpu_push(vdl2gpu_ctx *c, uint32_t r, const void *iq, uint32_t
 	return VDL2GPU_OK;
 }
 
-/* vdl2gpu_update_receivers: rings for the new list n beside the old ones in c, each kept receiver's queue moved to its new
- * index: its partial group (fewer bytes than a group, read from the host mirror of its old ring, written at the same stream
- * positions of its new ring) and its arrival and span records.  c is left as it was. */
-static int carry_pushed(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const int32_t *from) {
-	int rc = alloc_rings(n);
-	for(uint32_t r = 0; r < n->n_streams && rc == VDL2GPU_OK; r++) {
+/* vdl2gpu_update_receivers: rings P for the new layout n beside the old ones in c, each kept receiver's queue moved to its
+ * new index: its partial group (fewer bytes than a group, read from the host mirror of its old ring, written at the same
+ * stream positions of its new ring) and its arrival and span records.  c is left as it was. */
+static int carry_pushed(vdl2gpu_ctx *c, const ctx_layout &n, const int32_t *from, push_rings &P) {
+	int rc = alloc_rings(P, n, c->cfg.max_chunk_bytes);
+	for(uint32_t r = 0; r < n.n_streams && rc == VDL2GPU_OK; r++) {
 		if(from[r] < 0) continue;
-		push_rx &o = *c->push[from[r]], &q = *n->push[r];
+		push_rx &o = *c->push[from[r]], &q = *P.push[r];
 		q.head = o.head; q.tail = q.freed = o.tail;
 		q.recs = o.recs; q.anchors = o.anchors;
 		std::vector<uint8_t> part;
 		const vdl2_rx_ring &rg = c->rings[from[r]];
 		const vdl2_ring_segs sg = vdl2_ring_segments(rg.cap, o.tail, o.head - o.tail);
 		for(int k = 0; k < 2; k++) part.insert(part.end(), c->h_rings + rg.base + sg.off[k], c->h_rings + rg.base + sg.off[k] + sg.len[k]);
-		rc = ring_write(n, c->s_copy, r, q.tail, part.data(), (uint32_t)part.size());
+		rc = ring_write(P, c->s_copy, r, q.tail, part.data(), (uint32_t)part.size());
 	}
-	if(rc == VDL2GPU_OK) { cudaError_t e = cudaStreamSynchronize(c->s_copy); if(e != cudaSuccess) rc = fail_cuda(e, "cudaStreamSynchronize", __LINE__); }
-	if(rc) free_rings(n);
-	else n->push_ready = true;
+	/* also on failure: P's buffers may go only once their copies are done */
+	const cudaError_t e = cudaStreamSynchronize(c->s_copy);
+	if(rc == VDL2GPU_OK && e != cudaSuccess) rc = fail_cuda(e, "cudaStreamSynchronize", __LINE__);
 	return rc;
-}
-
-/* exchange the pushed-input rings (the switch of vdl2gpu_update_receivers; the copy stream stays with the context) */
-static void swap_rings(vdl2gpu_ctx *a, vdl2gpu_ctx *b) {
-	using std::swap;
-	swap(a->d_rings, b->d_rings); swap(a->h_rings, b->h_rings); swap(a->rings, b->rings); swap(a->d_ring_tab, b->d_ring_tab);
-	swap(a->push, b->push);
-	const bool pa = a->push_ready, pb = b->push_ready;
-	a->push_ready = pb; b->push_ready = pa;
 }
 
 /* decimated samples before a receiver's position for which span and arrival records are kept: a burst is harvested at
@@ -1593,16 +1545,10 @@ extern "C" int vdl2gpu_restart_receiver(vdl2gpu_ctx *c, uint32_t r, uint32_t cen
 	return VDL2GPU_OK;
 }
 
-/* device memory freed on every way out of vdl2gpu_update_receivers */
-struct dev_scratch {
-	void *p = nullptr;
-	~dev_scratch() { cudaFree(p); }
-};
-
 /* vdl2gpu_update_receivers once everything is checked: the new layout n (setup_layout) is filled from the old one in c.
  * Only n's buffers are written; c's are read. */
-static int migrate_receivers(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const vdl2gpu_receiver_ex *rx, const int32_t *from) {
-	const uint32_t n_rx = n->n_streams;
+static int migrate_receivers(vdl2gpu_ctx *c, ctx_layout &n, const vdl2gpu_receiver_ex *rx, const int32_t *from) {
+	const uint32_t n_rx = n.n_streams;
 	CU(cudaStreamSynchronize(c->stream));
 	CU(cudaStreamSynchronize(c->s_back));
 	vdl2_queue_ctl ctl;
@@ -1613,47 +1559,47 @@ static int migrate_receivers(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const vdl2gpu_recei
 	}
 	std::vector<uint32_t> old_slot_of_burst(c->n_chp);          /* K2_SLOT of every old slot: the pool slot its burst in progress holds */
 	CU(cudaMemcpy(old_slot_of_burst.data(), c->d_k2 + (size_t)K2_SLOT * c->n_chp, c->n_chp * 4, cudaMemcpyDeviceToHost));
-	std::vector<vdl2_rx_migrate> map(n->n_chp);
-	std::vector<uint8_t> held(n->n_slots, 0);
-	for(uint32_t i = 0; i < n->n_chp; i++) {
+	std::vector<vdl2_rx_migrate> map(n.n_chp);
+	std::vector<uint8_t> held(n.n_slots, 0);
+	for(uint32_t i = 0; i < n.n_chp; i++) {
 		vdl2_rx_migrate &m = map[i];
 		memset(&m, 0, sizeof(m));
-		m.slot_from = vdl2_rx_slot_from(i, n->lanes, n->full_warps, n->n_ch, n->rx_first.data(), n_rx, from, c->lanes, c->full_warps,
+		m.slot_from = vdl2_rx_slot_from(i, n.lanes, n.full_warps, n.n_ch, n.rx_first.data(), n_rx, from, c->lanes, c->full_warps,
 				c->rx_first.data());
-		m.chan_from = i < n->n_ch ? vdl2_rx_chan_from(i, n->rx_first.data(), n_rx, from, c->rx_first.data()) : -1;
+		m.chan_from = i < n.n_ch ? vdl2_rx_chan_from(i, n.rx_first.data(), n_rx, from, c->rx_first.data()) : -1;
 		uint32_t chan;
-		if(!vdl2_slot_channel(i, n->lanes, n->full_warps, n->n_ch, chan)) continue;
-		const uint32_t r = n->ch_rx[chan];
+		if(!vdl2_slot_channel(i, n.lanes, n.full_warps, n.n_ch, chan)) continue;
+		const uint32_t r = n.ch_rx[chan];
 		if(m.slot_from >= 0) {
 			m.hist_row = c->rx_prev[from[r]];
 			const int32_t b = (int32_t)old_slot_of_burst[m.slot_from];
 			if(b >= 0) held[b] = 1;                               /* (b < old n_slots <= n_slots: the index stays valid) */
 		} else {
-			m.dphi = vdl2_nco_dphi(rx[r].centerfreq, n->freqs[chan], (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * rx[r].oversample);
-			m.freq = n->freqs[chan];
+			m.dphi = vdl2_nco_dphi(rx[r].centerfreq, n.freqs[chan], (uint32_t)VDL2_SYMBOL_RATE * VDL2_SPS * rx[r].oversample);
+			m.freq = n.freqs[chan];
 		}
 	}
 	/* the free list: every pool slot no kept channel holds (those of removed receivers come back) */
 	std::vector<int32_t> fl;
-	fl.reserve(n->n_slots);
-	for(uint32_t i = 0; i < n->n_slots; i++) if(!held[i]) fl.push_back((int32_t)i);
+	fl.reserve(n.n_slots);
+	for(uint32_t i = 0; i < n.n_slots; i++) if(!held[i]) fl.push_back((int32_t)i);
 	ctl.free_top = (int32_t)fl.size();
-	dev_scratch d_map;
-	CU(cudaMalloc(&d_map.p, map.size() * sizeof(vdl2_rx_migrate)));
-	CU(cudaMemcpy(d_map.p, map.data(), map.size() * sizeof(vdl2_rx_migrate), cudaMemcpyHostToDevice));
+	dev_mem<vdl2_rx_migrate> d_map;
+	CU(cudaMalloc(d_map.put(), map.size() * sizeof(vdl2_rx_migrate)));
+	CU(cudaMemcpy(d_map, map.data(), map.size() * sizeof(vdl2_rx_migrate), cudaMemcpyHostToDevice));
 	/* the plane the next span takes its history from: the other one of its own (run_chain) */
 	const int pb_prev = (int)((c->chunk_seq & 1u) ^ 1u);
 	vdl2_migrate_params p;
-	p.map = static_cast<const vdl2_rx_migrate *>(d_map.p);
-	p.n_chp = n->n_chp; p.old_n_chp = c->n_chp;
+	p.map = d_map;
+	p.n_chp = n.n_chp; p.old_n_chp = c->n_chp;
 	p.old_k1 = c->d_k1; p.old_k2 = c->d_k2; p.old_counters = c->d_counters; p.old_ring = c->d_ring; p.old_phase = c->d_phase2[pb_prev];
-	p.k1 = n->d_k1; p.k2 = n->d_k2; p.counters = n->d_counters; p.ring = n->d_ring; p.phase = n->d_phase2[pb_prev];
-	p.old_chlv = c->d_chlv; p.chlv = n->d_chlv;                  /* (channel levels: both NULL or both allocated) */
+	p.k1 = n.d_k1; p.k2 = n.d_k2; p.counters = n.d_counters; p.ring = n.d_ring; p.phase = n.d_phase2[pb_prev];
+	p.old_chlv = c->d_chlv; p.chlv = n.d_chlv;                  /* (channel levels: both NULL or both allocated) */
 	KL(vdl2_launch_migrate(&p, c->stream));
 	/* held slots keep their indices (and their words): K2 writes a burst's channel number into its slot only at hand-off */
-	CU(cudaMemcpyAsync(n->d_pool, c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot), cudaMemcpyDeviceToDevice, c->stream));
-	CU(cudaMemcpyAsync(n->d_free, fl.data(), fl.size() * 4, cudaMemcpyHostToDevice, c->stream));
-	CU(cudaMemcpyAsync(n->d_ctl, &ctl, sizeof(ctl), cudaMemcpyHostToDevice, c->stream));
+	CU(cudaMemcpyAsync(n.d_pool, c->d_pool, (size_t)c->n_slots * sizeof(vdl2_burst_slot), cudaMemcpyDeviceToDevice, c->stream));
+	CU(cudaMemcpyAsync(n.d_free, fl.data(), fl.size() * 4, cudaMemcpyHostToDevice, c->stream));
+	CU(cudaMemcpyAsync(n.d_ctl, &ctl, sizeof(ctl), cudaMemcpyHostToDevice, c->stream));
 	/* input levels: a kept receiver carries its accumulator to its new index, a new one starts at zero (setup_layout) */
 	std::vector<vdl2_levels> old_lv, new_lv;
 	if(c->d_levels) {
@@ -1662,22 +1608,22 @@ static int migrate_receivers(vdl2gpu_ctx *c, vdl2gpu_ctx *n, const vdl2gpu_recei
 		CU(cudaMemcpyAsync(old_lv.data(), c->d_levels, old_lv.size() * sizeof(vdl2_levels), cudaMemcpyDeviceToHost, c->stream));
 		CU(cudaStreamSynchronize(c->stream));
 		for(uint32_t r = 0; r < n_rx; r++) if(from[r] >= 0) new_lv[r] = old_lv[from[r]];
-		CU(cudaMemcpyAsync(n->d_levels, new_lv.data(), new_lv.size() * sizeof(vdl2_levels), cudaMemcpyHostToDevice, c->stream));
+		CU(cudaMemcpyAsync(n.d_levels, new_lv.data(), new_lv.size() * sizeof(vdl2_levels), cudaMemcpyHostToDevice, c->stream));
 	}
 	/* spectrum: likewise, with its waiting samples and its place on its segment grid */
 	if(c->d_spec)
 		for(uint32_t r = 0; r < n_rx; r++) {
 			if(from[r] < 0) continue;
-			CU(cudaMemcpyAsync(n->d_spec + r, c->d_spec + from[r], sizeof(vdl2_spec_acc), cudaMemcpyDeviceToDevice, c->stream));
-			n->spec_pos[r] = c->spec_pos[from[r]];
+			CU(cudaMemcpyAsync(n.d_spec + r, c->d_spec + from[r], sizeof(vdl2_spec_acc), cudaMemcpyDeviceToDevice, c->stream));
+			n.spec_pos[r] = c->spec_pos[from[r]];
 		}
 	CU(cudaStreamSynchronize(c->stream));
 	/* per receiver: a kept one carries its position and a pending restart over; every history now starts at row 0 */
 	for(uint32_t r = 0; r < n_rx; r++) {
 		if(from[r] < 0) continue;
-		n->rx_pos[r] = c->rx_pos[from[r]];
-		n->rx_restart_pending[r] = c->rx_restart_pending[from[r]];
-		n->n_restart_pending += n->rx_restart_pending[r];
+		n.rx_pos[r] = c->rx_pos[from[r]];
+		n.rx_restart_pending[r] = c->rx_restart_pending[from[r]];
+		n.n_restart_pending += n.rx_restart_pending[r];
 	}
 	return VDL2GPU_OK;
 }
@@ -1727,26 +1673,19 @@ extern "C" int vdl2gpu_update_receivers(vdl2gpu_ctx *c, const vdl2gpu_receiver_e
 	cfg.n_streams = n_rx;
 	std::vector<vdl2gpu_receiver> base(n_rx);
 	for(uint32_t r = 0; r < n_rx; r++) { base[r].centerfreq = rx[r].centerfreq; base[r].n_channels = rx[r].n_channels; }
-	vdl2gpu_ctx *n = new vdl2gpu_ctx();
-	n->cfg = c->cfg;
-	n->device = c->device; n->n_sms = c->n_sms;
-	n->receivers = n->mixed = n->ragged = true;
-	n->n_streams = n_rx;
-	n->cfg.n_streams = n_rx;
-	int rc = setup_layout(n, &cfg, base.data(), n_rx, rx, c->n_slots, "vdl2gpu_update_receivers");
+	ctx_layout n;
+	push_rings p;
+	int rc = setup_layout(n, cfg, base.data(), n_rx, rx, true, true, true, false, c->n_sms, c->n_slots, "vdl2gpu_update_receivers");
 	if(rc == VDL2GPU_OK) rc = migrate_receivers(c, n, rx, from);
-	if(rc == VDL2GPU_OK && c->push_ready) rc = carry_pushed(c, n, from);
-	if(rc == VDL2GPU_OK) {
-		swap_layout(c, n);
-		swap_rings(c, n);
-		/* the graphs went with the old chunk slots: the next spans capture anew, as after create */
-		c->graph_nominal = 0;
-		c->last_n_dec = 0;
-	}
-	free_rings(n);
-	free_layout(n);
-	delete n;
-	return rc;
+	if(rc == VDL2GPU_OK && c->push_ready) rc = carry_pushed(c, n, from, p);
+	if(rc) return rc;
+	/* the switch: the old layout and rings go with n and p, the graphs with the old chunk slots (the next spans capture
+	 * anew, as after create) */
+	std::swap(static_cast<ctx_layout &>(*c), n);
+	if(c->push_ready) std::swap(static_cast<push_rings &>(*c), p);
+	c->graph_nominal = 0;
+	c->last_n_dec = 0;
+	return VDL2GPU_OK;
 }
 
 extern "C" int vdl2gpu_get_receiver_positions(vdl2gpu_ctx *c, uint64_t *out, uint32_t n_rx) {
@@ -2038,7 +1977,7 @@ extern "C" int vdl2gpu_read_events(vdl2gpu_ctx *c, vdl2gpu_event *out, uint32_t 
 		if(ctl.n_events > c->event_cap) c->events_dropped += ctl.n_events - c->event_cap;
 		if(ctl.n_events) {
 			const uint32_t zero = 0;
-			CU(cudaMemcpy(reinterpret_cast<uint8_t *>(c->d_ctl) + offsetof(vdl2_queue_ctl, n_events), &zero, sizeof(zero), cudaMemcpyHostToDevice));
+			CU(cudaMemcpy(reinterpret_cast<uint8_t *>(c->d_ctl.get()) + offsetof(vdl2_queue_ctl, n_events), &zero, sizeof(zero), cudaMemcpyHostToDevice));
 			c->events_read = 0;
 		}
 	}
@@ -2055,7 +1994,7 @@ extern "C" int vdl2gpu_enable_timing(vdl2gpu_ctx *c, int on) {
 	c->timing = on != 0;
 	if(on && !c->ev_t0) {
 		CU(cudaSetDevice(c->device));
-		CU(cudaEventCreate(&c->ev_t0));
+		CU(cudaEventCreate(c->ev_t0.put()));
 		CU(cudaEventRecord(c->ev_t0, c->stream));
 	}
 	return VDL2GPU_OK;
